@@ -1,4 +1,4 @@
-"""alpa_b200: a B200-native auto-parallel training and serving framework with the capabilities of
+"""alpa_b200: a H100-native auto-parallel training and serving framework with the capabilities of
 alpa-projects/alpa (reference public surface: alpa/__init__.py:22-51)."""
 from alpa_b200.version import __version__  # noqa: F401
 from alpa_b200.global_env import global_config  # noqa: F401

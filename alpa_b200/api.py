@@ -3,7 +3,7 @@
 Reference: alpa/api.py (init:25, shutdown:63, parallelize:71, ParallelizedFunc:106, grad:241,
 value_and_grad:265).  The decorated function is ordinary PyTorch code over pytrees of tensors; it is
 traced once per input signature into a flat graph (forward + backward + optimizer), planned, lowered
-to a per-rank SPMD program of sm_100a kernels + collectives, and cached.
+to a per-rank SPMD program of sm_90a kernels + collectives, and cached.
 """
 from __future__ import annotations
 

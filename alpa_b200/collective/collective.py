@@ -4,7 +4,7 @@ Reference: alpa/collective/collective.py (GroupManager:74, init_collective_group
 allreduce:261 ... send:566, recv:629, _check_and_get_group:734) with NCCL/Gloo backends implemented on cupy / pygloo
 (collective_group/*.py), stream pools (cuda_stream.py) and a Ray-actor rendezvous.
 
-B200 design: one process per GPU already shares a `torch.distributed` world (NCCL over NVLink/NVSwitch; gloo on
+H100 design: one process per GPU already shares a `torch.distributed` world (NCCL over NVLink/NVSwitch; gloo on
 CPU hosts), so a named group is a `dist.new_group` handle plus the rank translation table.  Rendezvous is the
 world's store -- no actors.  P2P between two ranks uses batched isend/irecv (one NCCL group launch per direction,
 like the reference's 2-rank communicators, without creating a communicator per GPU pair).  Collectives that have

@@ -1,10 +1,10 @@
 """Fused compute + collective operators over NVLink peer memory (symmetric memory).
 
-These are the B200-native replacements for "cuBLAS GEMM then NCCL collective" (the reference's K3/K5:
+These are the H100-native replacements for "cuBLAS GEMM then NCCL collective" (the reference's K3/K5:
 out-projection / MLP-down GEMM followed by all-reduce or reduce-scatter, and K1/K4: all-gather followed by
 the QKV / MLP-up GEMM; XLA/service/gpu/nccl_all_reduce_thunk.cc:103-121,:434-458, nccl_all_gather_thunk.cc).
 
-* ``FusedLinearReduceScatter``: y_shard = reduce_scatter(x_local @ w_local^T).  The tcgen05 GEMM epilogue
+* ``FusedLinearReduceScatter``: y_shard = reduce_scatter(x_local @ w_local^T).  The GEMM epilogue
   stores every partial tile directly into the owning GPU's staging buffer (peer store over NVLink) and
   bumps an arrival counter; a small reduce kernel on the owner sums the tp slots (+bias, +residual).
 * ``FusedAllGatherLinear``: y = all_gather(x_shard) @ w_local^T.  A push kernel on a side stream writes the

@@ -177,8 +177,9 @@ static bool strategy_allowed(const Node& n, const MeshEnv& env, const Options& o
   return true;
 }
 
-// Measured B200 ratio between tensor-core math and NVLink traffic: ~1.4e15 FLOP/s against ~7.7e11 B/s.
-constexpr double kFlopsPerCommUnit = 1800.0;
+// Ratio between tensor-core math and NVLink traffic on the H100 SXM from data-sheet rates: 989e12 dense bf16 FLOP/s
+// against 4.5e11 B/s per direction of NVLink 4 (~2200 FLOP per byte moved).
+constexpr double kFlopsPerCommUnit = 2200.0;
 
 // Reference: AnnotateShardingWithSimpleHeuristic (auto_sharding_util.cc:2017-2110): program inputs are laid out by a
 // rule of thumb -- the largest / first / last dim tiled over the mesh (the two largest dims on a 2-D mesh for

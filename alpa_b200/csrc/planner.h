@@ -1,6 +1,6 @@
 // alpa_b200 native planner: op-graph IR, sharding strategies, cost graph, ILP assembly.
 //
-// This is the B200-native equivalent of the reference's C++ auto-sharding pass
+// This is the H100-native equivalent of the reference's C++ auto-sharding pass
 // (XLA/service/spmd/auto_sharding.cc, auto_sharding_strategy.h, auto_sharding_dot_handler.cc,
 // auto_sharding_util.cc).  Instead of per-HLO-opcode handlers, every op is described by an
 // einsum-like *label signature*: each operand/output dim carries a label; a strategy is an

@@ -4,7 +4,7 @@ Reference: alpa/data_loader.py (DataLoader:15 -- driver-side iterator with a pre
 batch according to the executable's input placement specs; MeshDriverDataLoader:97 / MeshWorkerDataLoader:229 --
 every host loads only the slice of the global batch that its own devices need).
 
-B200 design: one process per GPU, so "each host loads its slice" becomes "each rank reads the rows its device's
+H100 design: one process per GPU, so "each host loads its slice" becomes "each rank reads the rows its device's
 shard covers".  Batches are staged in pinned host memory and copied on a dedicated CUDA copy stream, `prefetch_size`
 batches ahead, so the H2D copy of step i+1 overlaps the compute of step i; consumers wait on the copy event only.
 """

@@ -4,11 +4,11 @@ Reference: alpa/device_mesh.py (DeviceCluster:2131, VirtualPhysicalMesh:1792, Ph
 LocalPhysicalDeviceMesh:860, DistributedPhysicalDeviceMesh:979, DistributedArray:1509,
 ReplicatedDistributedArray:1697, PhysicalDeviceMeshGroup:1979, globals :2308-2406).
 
-B200-native process model: **one process per GPU, SPMD** (torchrun / mp.spawn), no Ray driver and no
+H100-native process model: **one process per GPU, SPMD** (torchrun / mp.spawn), no Ray driver and no
 remote buffer table -- every rank runs the same Python program, owns the shards of its own GPU and
 executes the same statically planned program.  Two execution backends share one executor:
 
-* ``DistCommunicator``     -- real multi-process meshes over ``torch.distributed`` (nccl on B200,
+* ``DistCommunicator``     -- real multi-process meshes over ``torch.distributed`` (nccl on GPUs,
                               gloo on CPU); each process has exactly one local device.
 * ``EmulatedCommunicator`` -- all logical devices live in this process (a list of shards per array);
                               used by ``cluster="local"`` with ``num_devices>1`` and by device-free

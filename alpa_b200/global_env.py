@@ -1,6 +1,6 @@
 """Global configuration (one mutable object, like the reference's alpa/global_env.py:5-139).
 
-Differences that follow from the B200-native design: there is no XLA/Ray, so the XLA memory and
+Differences that follow from the H100-native design: there is no XLA/Ray, so the XLA memory and
 port knobs are replaced by torch.distributed / CUDA-graph / symmetric-memory knobs; every option the
 reference exposes for the planner and the pipeline runtime keeps its name.
 """
@@ -23,7 +23,7 @@ class GlobalConfig:
         self.compile_random_seed = 42
         self.runtime_random_seed = 42
         self.delete_remote_arrays_threshold = 50
-        # Compute dtype policy of the kernel library: bf16 tensors run the sm_100a kernels,
+        # Compute dtype policy of the kernel library: bf16 tensors run the sm_90a kernels,
         # everything else (CPU, fp32) runs the PyTorch reference implementation of the same op.
         self.use_native_kernels = True
         # If True the ops refuse to fall back to PyTorch on a CUDA device (used by bench/tests to

@@ -4,7 +4,8 @@ Reference: alpa/mesh_profiling.py (MeshProfilingResult:18, ProfilingResultDataba
 enumerate_all_collective_spec:668, profile_all:725, estimate_hlo_module_cost:901) and the C++ HLO cost model
 (XLA/service/gpu/gpu_cost_model.cc).  The reference micro-benchmarks XLA executables (dot, all-reduce,
 all-gather, reduce-scatter, all-to-all) and interpolates; here the same tables are filled by timing *our*
-kernels and NCCL collectives with CUDA events, and the B200 defaults come from MEASURED_PEAKS.json.
+kernels and NCCL collectives with CUDA events; without them the H100 data-sheet defaults of `CostModel` apply,
+overridden by a measured MEASURED_PEAKS.json when one is present.
 """
 from __future__ import annotations
 
@@ -150,16 +151,17 @@ class ProfilingResultDatabase:
 
 
 # ------------------------------------------------------------------------------------------------
-# analytic model (defaults = this pool's measured B200 numbers)
+# analytic model.  Defaults are NVIDIA data-sheet figures of the H100 SXM (80 GB HBM3, 700 W), not measurements:
+# peak rates are upper bounds, so a measured MEASURED_PEAKS.json (or a profiled database) replaces them when present.
 # ------------------------------------------------------------------------------------------------
 @dataclass
 class CostModel:
-    flops_per_second: float = 1.4e15          # sustained bf16 GEMM (MEASURED_PEAKS.json)
-    hbm_bytes_per_second: float = 6.5e12
-    nvlink_bytes_per_second: float = 7.7e11   # per direction per GPU (B200_PROFILING.md)
-    allreduce_bus_bytes_per_second: float = 7.25e11
-    collective_latency: float = 12e-6
-    memory_bytes: float = 180e9
+    flops_per_second: float = 989e12          # dense bf16 tensor-core peak (data sheet)
+    hbm_bytes_per_second: float = 3.35e12     # HBM3 (data sheet)
+    nvlink_bytes_per_second: float = 4.5e11   # NVLink 4: 900 GB/s bidirectional = 450 GB/s per direction per GPU
+    allreduce_bus_bytes_per_second: float = 4.5e11   # bus bandwidth bound by the per-direction link rate
+    collective_latency: float = 12e-6         # assumed per-collective launch + synchronisation latency
+    memory_bytes: float = 80e9                # HBM capacity per GPU
 
     def all_reduce_seconds(self, num_bytes: float, n: int) -> float:
         if n <= 1:
@@ -224,8 +226,8 @@ def default_cost_model() -> CostModel:
         try:
             with open(path) as f:
                 p = json.load(f)
-            cm.flops_per_second = float(p.get("bf16_tflops_sustained", 1400.0)) * 1e12
-            cm.hbm_bytes_per_second = float(p.get("hbm_gbs", 6500.0)) * 1e9
+            cm.flops_per_second = float(p.get("bf16_tflops_sustained", cm.flops_per_second / 1e12)) * 1e12
+            cm.hbm_bytes_per_second = float(p.get("hbm_gbs", cm.hbm_bytes_per_second / 1e9)) * 1e9
         except Exception:  # noqa: BLE001
             pass
         _default_cm = cm
@@ -238,7 +240,7 @@ def set_cost_model(cm: CostModel):
 
 
 # ------------------------------------------------------------------------------------------------
-# on-device profiling (run inside a torchrun job on the B200 box)
+# on-device profiling (run inside a torchrun job on the GPU node)
 # ------------------------------------------------------------------------------------------------
 def _time_cuda(fn, warmup=3, iters=10) -> float:
     for _ in range(warmup):
@@ -282,7 +284,7 @@ def enumerate_collective_specs(group_size: int, max_comm_size_log2: int, min_com
 def profile_one_mesh(group_ranks: Sequence[int], max_comm_size_log2: int = 28, dot_sizes=(1024, 2048, 4096, 8192),
                      skip_keys: Optional[set] = None, max_retry: int = 2, min_comm_size_log2: int = 10,
                      dtypes: Sequence[str] = ("bf16", "f32")) -> MeshProfilingResult:
-    """Time bf16 GEMMs (our tcgen05 kernel) and the collectives of `enumerate_collective_specs` over `group_ranks`
+    """Time bf16 GEMMs (our wgmma kernel) and the collectives of `enumerate_collective_specs` over `group_ranks`
     (reference: profile_one_hlo_op / profile_hlo_ops, mesh_profiling.py:392-665).  Every measurement is retried up to
     `max_retry` times; one that keeps failing (out of memory at the largest sizes, an unsupported dtype on a backend)
     is recorded in `failed_keys` and skipped -- the profile of the mesh still completes.  Keys in `skip_keys` (failures
@@ -428,6 +430,6 @@ estimate_hlo_module_cost = estimate_stage_cost_from_db
 
 
 def profile_dot(sizes=(1024, 2048, 4096, 8192)):
-    """[(flops, seconds)] of square bf16 GEMMs with this package's tcgen05 kernel (reference: profile_dot)."""
+    """[(flops, seconds)] of square bf16 GEMMs with this package's wgmma kernel (reference: profile_dot)."""
     res = profile_one_mesh([0], max_comm_size_log2=0, dot_sizes=tuple(sizes))
     return res.dot_cost_dict.get(("bf16",), [])

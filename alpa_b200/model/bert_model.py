@@ -4,7 +4,7 @@ Reference: alpa/model/bert_model.py (BertConfig:27, FlaxBertEmbeddings:110, Flax
 FlaxBertLayer:338, FlaxBertLayerCollection:380, FlaxBertEncoder:437, FlaxBertPooler:461, FlaxBertLMPredictionHead:
 497, FlaxBertForPreTraining / ForMaskedLM / ForSequenceClassification :556-884).  Same post-LN architecture; the
 encoder layer is `GPTBlock` (fused QKV GEMM, packed flash attention, GELU in the GEMM epilogue, residual fused into
-LayerNorm).  A padding mask disables the flash kernel for that call (the sm_100a attention kernel supports full and
+LayerNorm).  A padding mask disables the flash kernel for that call (the sm_90a attention kernel supports full and
 causal masks); padded batches run the composed softmax path with identical maths.
 """
 from __future__ import annotations

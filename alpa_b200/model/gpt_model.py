@@ -6,7 +6,7 @@ residual+LayerNorm, dense+GELU, dense, residual+LayerNorm] (post-LN) -> vocabula
 The reference attends bidirectionally with an all-ones mask in its GPT benchmark
 (benchmark_one_case_gpt_bert.py:142-148); `causal=True` gives the usual decoder masking.
 
-B200 mapping: fused QKV projection (features ordered (head, {q,k,v}, D) so tensor-parallel splits are
+H100 mapping: fused QKV projection (features ordered (head, {q,k,v}, D) so tensor-parallel splits are
 head splits), packed flash attention, GELU / bias / pre-activation fused into GEMM epilogues,
 residual-add fused into LayerNorm, per-token fused cross-entropy.
 """

@@ -102,7 +102,7 @@ class SGD(Optimizer):
 
 
 class Adam(Optimizer):
-    """Adam / AdamW on fp32 state.  fused=True runs the single-launch sm_100a multi-tensor kernel in
+    """Adam / AdamW on fp32 state.  fused=True runs the single-launch sm_90a multi-tensor kernel in
     place (requires the train state to be donated); fused=False is plain traceable torch math."""
 
     def __init__(self, learning_rate: float, b1: float = 0.9, b2: float = 0.999, eps: float = 1e-8,
@@ -258,7 +258,7 @@ pytree.register_pytree_node(
 class TrainState:
     """Parameters + optimizer state (+ optional fp32 master copy) as one pytree.
 
-    Reference: alpa/model/model_util.py:273-378.  `params` are in the compute dtype (bf16 on B200);
+    Reference: alpa/model/model_util.py:273-378.  `params` are in the compute dtype (bf16 on the GPU);
     with `use_master_copy` the optimizer runs on `master_copy` (fp32) and refreshes `params`."""
 
     def __init__(self, step, params, opt_state, master_copy=None, dynamic_scale=None, apply_fn=None, tx=None):

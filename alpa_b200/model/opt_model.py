@@ -5,7 +5,7 @@ KV cache threaded through `attention_cache`, OPTTransformerLayer:316, OPTForLMMo
 init_cache_np:756, load_params_np:875), bloom_model.py, codegen_model.py.  The reference compiles prompt ("encoder",
 chunked) and single-token ("decoder") executables with alpa's pipeshard runtime.
 
-B200 design: a dedicated SPMD inference engine -- one process per GPU, Megatron tensor parallelism written out
+H100 design: a dedicated SPMD inference engine -- one process per GPU, Megatron tensor parallelism written out
 explicitly (column-parallel QKV / FC1, row-parallel out-proj / FC2, vocab-parallel embedding and LM head), the
 all-reduces on the NVSwitch (NCCL / NVLS), KV cache resident in HBM as [B, S_max, heads_local, D] per layer, the
 prompt phase on the flash-attention kernel and every decode step replayed from a CUDA graph.  Weights can be kept in
@@ -97,7 +97,7 @@ class _TPLinear:
         self.fp8 = fp8 = bool(fp8) and not self.mx
         if self.mx:
             # OCP microscaling: e4m3 elements, one power-of-two scale per 32 input channels, stored in the scale-atom
-            # layout of tcgen05.mma.kind::mxf8f6f4.block_scale (opt-in: the kernel has not had a hardware run yet)
+            # layout read by the MXFP8 GEMM (opt-in: the kernel has not had a hardware run yet)
             self.w, self.scale = ops.quantize_mxfp8(w.contiguous())
         elif fp8:
             amax = w.float().abs().amax(dim=1).clamp(min=1e-8)

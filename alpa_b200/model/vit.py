@@ -2,8 +2,8 @@
 
 Reference: examples/ViT/run_image_classification.py fine-tunes HuggingFace's FlaxViTForImageClassification under
 alpa.parallelize; the model itself comes from `transformers`.  Here the encoder is built from the framework's own
-fused transformer block (alpa_b200.model.gpt_model.GPTBlock: tcgen05 GEMMs with fused bias/GELU epilogues, flash
-attention, fused add+LayerNorm), so every ViT matmul runs on the sm_100a kernels and the auto-sharding planner sees
+fused transformer block (alpa_b200.model.gpt_model.GPTBlock: wgmma GEMMs with fused bias/GELU epilogues, flash
+attention, fused add+LayerNorm), so every ViT matmul runs on the sm_90a kernels and the auto-sharding planner sees
 the same operator set as for GPT/BERT.  Patch embedding is the strided convolution written as unfold + GEMM.
 """
 from __future__ import annotations

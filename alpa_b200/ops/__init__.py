@@ -2,7 +2,7 @@
 
 Every primitive is a ``torch.library`` custom op in the ``alpa_b200`` namespace with
 
-* a CUDA/bf16 implementation backed by the hand-written sm_100a kernels in ``ops/csrc`` (``_C``),
+* a CUDA/bf16 implementation backed by the hand-written sm_90a kernels in ``ops/csrc`` (``_C``),
 * a plain PyTorch reference implementation of the same maths (CPU, fp32, and the numerics oracle),
 * a fake (meta) implementation so train steps can be traced without touching a device,
 * an autograd formula expressed in other primitives (so fwd+bwd trace to one flat graph), and

@@ -1,12 +1,12 @@
 """In-tree build of the alpa_b200 native libraries.
 
-Two shared objects are produced next to this file (git-ignored, shipped to GPU boxes by gpurun):
+Two shared objects are produced next to this file (git-ignored):
 
-* ``_C*.so``       -- sm_100a CUDA kernels + torch bindings  (``alpa_b200/ops/csrc``)
+* ``_C*.so``       -- sm_90a CUDA kernels + torch bindings  (``alpa_b200/ops/csrc``)
 * ``_planner*.so`` -- C++ planner / runtime core (auto-sharding strategy enumeration, cost graph,
                       ILP branch-and-bound, inter-op DP, instruction interpreter)  (``alpa_b200/csrc``)
 
-Kernels are compiled with ``nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo`` (cross-compiles
+Kernels are compiled with ``nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo`` (cross-compiles
 on a CPU-only box); the binding translation units with g++.  Objects are cached by content hash.
 """
 from __future__ import annotations
@@ -26,13 +26,13 @@ PLANNER_SRC = PKG_DIR / "csrc"
 BUILD_DIR = PKG_DIR.parent / "build"
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-# NOTE: $CXX in this image points at a wrapper that links libstdc++ statically, which clashes with
+# NOTE: $CXX may point at a wrapper that links libstdc++ statically, which clashes with
 # torch's libstdc++ inside one process; always use the system g++ unless explicitly overridden.
 CXX = os.environ.get("ALPA_B200_CXX", "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++")
 CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "--use_fast_math",
 ]
 

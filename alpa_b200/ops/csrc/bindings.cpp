@@ -1,4 +1,4 @@
-// Python bindings for the alpa_b200 sm_100a kernel library (torch tensors in, raw pointers out).
+// Python bindings for the alpa_b200 sm_90a kernel library (torch tensors in, raw pointers out).
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
@@ -9,7 +9,7 @@
 #include <unordered_map>
 #include <vector>
 
-#include "gemm_sm100.h"
+#include "gemm_sm90.h"
 #include "kernels.h"
 
 namespace {
@@ -98,22 +98,7 @@ Tensor gemm(const Tensor& a, const Tensor& b, bool trans_a, bool trans_b, const 
   g.ep.residual = bf16_ptr(residual);
   g.ep.aux_out = const_cast<__nv_bfloat16*>(bf16_ptr(aux_out));
   g.ep.aux_in = bf16_ptr(aux_in);
-  // CTA-pair kernel (gemm2_sm100.cu): block_n == 2 forces it; large 2-D GEMMs use it unless ALPA_B200_GEMM_2CTA=0
-  static const bool auto_2cta = [] {
-    const char* e = std::getenv("ALPA_B200_GEMM_2CTA");
-    return e == nullptr || e[0] != '0';      // default on: measured 5-17 % faster than the 1-CTA kernel on GPT shapes
-  }();
-  const bool want_2cta = block_n == 2 || (auto_2cta && block_n == 0 && nd == 2 && g.M >= 512 && g.N >= 256);
-  int rc;
-  if (want_2cta && nd == 2) {
-    g.block_n = 0;
-    rc = ab_gemm2_bf16(&g, cur_stream());
-    AB_CHECK_RC(rc, "ab_gemm2_bf16");
-  } else {
-    if (g.block_n == 2) g.block_n = 0;
-    rc = ab_gemm_bf16(&g, cur_stream());
-    AB_CHECK_RC(rc, "ab_gemm_bf16");
-  }
+  AB_CHECK_RC(ab_gemm_bf16(&g, cur_stream()), "ab_gemm_bf16");
   g_launches += 1;
   return out;
 }
@@ -245,7 +230,7 @@ void peer_barrier_auto(std::vector<int64_t> flag_ptrs, const Tensor& counter, in
   g_launches += 1;
 }
 
-// One-shot all-reduce of a small bf16 vector through a two-half symmetric staging buffer (see comm_sm100.cu).
+// One-shot all-reduce of a small bf16 vector through a two-half symmetric staging buffer (see comm_sm90.cu).
 void allreduce_oneshot(const Tensor& x, int64_t sym_local_ptr, int64_t mc_ptr, int64_t half_stride, Tensor out,
                        std::vector<int64_t> flag_ptrs, const Tensor& counter, int64_t rank, const OptTensor& residual) {
   uint32_t* flags[ab::kMaxPeersComm];
@@ -287,7 +272,7 @@ static void fill_attn_args(ab::AttnArgs& a, const Tensor& q, const Tensor& k, co
 
 // q,k,v: [B,S,h,D] (any strides with D contiguous, e.g. views of a fused QKV projection).
 std::vector<Tensor> attention_fwd(const Tensor& q, const Tensor& k, const Tensor& v, double scale,
-                                  bool causal, const OptTensor& kv_len, const OptTensor& trace) {
+                                  bool causal, const OptTensor& kv_len) {
   c10::cuda::CUDAGuard guard(q.device());
   ab::AttnArgs a;
   fill_attn_args(a, q, k, v, scale, causal);
@@ -296,39 +281,23 @@ std::vector<Tensor> attention_fwd(const Tensor& q, const Tensor& k, const Tensor
                 "attention: kv_len must be an int32 CUDA scalar");
     a.kv_len = kv_len->data_ptr<int>();
   }
-  if (trace.has_value() && trace->defined()) {
-    TORCH_CHECK(trace->is_cuda() && trace->scalar_type() == at::kLong && trace->numel() >= 1024, "attention: trace");
-    a.trace = reinterpret_cast<long long*>(trace->data_ptr<int64_t>());
-  }
   Tensor o = torch::empty({a.B, a.Sq, a.heads, a.D}, q.options());
   Tensor lse = torch::empty({a.B, a.heads, a.Sq}, q.options().dtype(at::kFloat));
   a.o = reinterpret_cast<__nv_bfloat16*>(o.data_ptr());
   a.lse = lse.data_ptr<float>();
   a.o_stride_b = o.stride(0); a.o_stride_s = o.stride(1); a.o_stride_h = o.stride(2);
-  // default: the persistent two-set kernel (gen 4) for head dim 64, the 16-warp kernel (gen 2) for every other head dim
-  // (measured, same lease: D = 64 S = 1024 0.147 vs 0.160 ms, causal 0.106 vs 0.123; D = 128 0.303 vs 0.252);
-  // a device-side KV length (prefill into a cache) keeps the first generation.  ALPA_B200_ATTN_FWD=gen2|gen3|gen4|legacy
-  // forces one.
-  static const std::string fwd_sel = [] {
+  // 128-query tiles by default; ALPA_B200_ATTN_FWD=gen2 pins the 64-query-tile configuration (twice the CTAs).  The
+  // kernel self-check (alpa_b200/ops/selfcheck.py) pins it when the default misbehaves on this GPU.
+  static const bool narrow = [] {
     const char* e = std::getenv("ALPA_B200_ATTN_FWD");
-    return std::string(e != nullptr ? e : "");
+    return e != nullptr && std::string(e) != "gen4";
   }();
-  const bool can4 = a.kv_len == nullptr && a.Skv >= a.Sq;
-  const bool use4 = can4 && (fwd_sel == "gen4" || (fwd_sel.empty() && a.D == 64));
-  if (use4) {
-    AB_CHECK_RC(ab_attention_fwd4(&a, cur_stream()), "ab_attention_fwd4");
-  } else if (a.kv_len == nullptr && fwd_sel == "gen3") {
-    AB_CHECK_RC(ab_attention_fwd3(&a, cur_stream()), "ab_attention_fwd3");
-  } else if (a.kv_len == nullptr && fwd_sel != "legacy") {
-    AB_CHECK_RC(ab_attention_fwd2(&a, cur_stream()), "ab_attention_fwd2");
-  } else {
-    AB_CHECK_RC(ab_attention_fwd(&a, cur_stream()), "ab_attention_fwd");
-  }
+  AB_CHECK_RC(ab_attention_fwd(&a, narrow ? 0 : 1, cur_stream()), "ab_attention_fwd");
   g_launches += 1;
   return {o, lse};
 }
 
-// Attention of a ragged 1-D token batch against a slot-addressed KV cache (see ragged_attention_sm100.cu).
+// Attention of a ragged 1-D token batch against a slot-addressed KV cache (see ragged_attention_sm90.cu).
 Tensor ragged_attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& seq_start,
                         const Tensor& ctx_len, double scale, int64_t max_ctx, const OptTensor& alibi) {
   TORCH_CHECK(q.dim() == 3 && q.stride(2) == 1 && q.scalar_type() == at::kBFloat16, "ragged_attention: q must be bf16 [T, heads, D]");
@@ -362,7 +331,7 @@ Tensor ragged_attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_
   return o;
 }
 
-// Sharding-invariant dropout: y = keep(seed, stream, global index) ? x / (1 - p) : 0   (dropout_sm100.cu)
+// Sharding-invariant dropout: y = keep(seed, stream, global index) ? x / (1 - p) : 0   (dropout_sm90.cu)
 Tensor dropout(const Tensor& x_in, double p, const Tensor& seed, int64_t stream, const std::vector<int64_t>& global_shape,
                const std::vector<int64_t>& offsets) {
   TORCH_CHECK(x_in.scalar_type() == at::kBFloat16 || x_in.scalar_type() == at::kFloat, "dropout: bf16 / fp32 only");
@@ -411,16 +380,7 @@ std::vector<Tensor> attention_bwd(const Tensor& d_o_in, const Tensor& q, const T
   a.f.o_stride_b = o.stride(0); a.f.o_stride_s = o.stride(1); a.f.o_stride_h = o.stride(2);
   a.d_o = bf16_ptr(d_o);
   const int B = a.f.B, H = a.f.heads, Sq = a.f.Sq, Skv = a.f.Skv, D = a.f.D;
-  // default: split dK/dV + dQ kernels (atomic-free, pipelined); ALPA_B200_ATTN_BWD=legacy selects the single kernel
-  // that reduces dQ with fp32 global atomics
-  static const bool legacy_env = [] {
-    const char* e = std::getenv("ALPA_B200_ATTN_BWD");
-    return e != nullptr && std::string(e) == "legacy";
-  }();
-  const bool legacy = legacy_env || (Sq % 4) != 0;   // the split kernels TMA-load per-query statistics rows (16-byte rows)
-  Tensor dq_acc;
-  if (legacy) dq_acc = torch::zeros({B, H, Sq, D}, q.options().dtype(at::kFloat));
-  Tensor delta = torch::empty({legacy ? 1 : 2, B, H, Sq}, q.options().dtype(at::kFloat));   // [-delta | -lse log2 e]
+  Tensor delta = torch::empty({B, H, Sq}, q.options().dtype(at::kFloat));
   auto pick = [&](const OptTensor& t, int S) {
     if (t.has_value() && t->defined()) {
       TORCH_CHECK(t->dim() == 4 && t->stride(3) == 1 && t->scalar_type() == at::kBFloat16 && t->size(1) == S);
@@ -429,20 +389,14 @@ std::vector<Tensor> attention_bwd(const Tensor& d_o_in, const Tensor& q, const T
     return torch::empty({B, S, H, D}, q.options());
   };
   Tensor dq = pick(dq_out, Sq), dk = pick(dk_out, Skv), dv = pick(dv_out, Skv);
-  a.dq_accum = legacy ? dq_acc.data_ptr<float>() : nullptr;
   a.delta = delta.data_ptr<float>();
-  a.nlse2 = legacy ? nullptr : delta.data_ptr<float>() + (size_t)B * H * Sq;
   a.dq = reinterpret_cast<__nv_bfloat16*>(dq.data_ptr());
   a.dk = reinterpret_cast<__nv_bfloat16*>(dk.data_ptr());
   a.dv = reinterpret_cast<__nv_bfloat16*>(dv.data_ptr());
   a.dq_stride_b = dq.stride(0); a.dq_stride_s = dq.stride(1); a.dq_stride_h = dq.stride(2);
   a.dk_stride_b = dk.stride(0); a.dk_stride_s = dk.stride(1); a.dk_stride_h = dk.stride(2);
   a.dv_stride_b = dv.stride(0); a.dv_stride_s = dv.stride(1); a.dv_stride_h = dv.stride(2);
-  if (legacy) {
-    AB_CHECK_RC(ab_attention_bwd(&a, cur_stream()), "ab_attention_bwd");
-  } else {
-    AB_CHECK_RC(ab_attention_bwd2(&a, cur_stream()), "ab_attention_bwd2");
-  }
+  AB_CHECK_RC(ab_attention_bwd(&a, cur_stream()), "ab_attention_bwd");
   g_launches += 3;
   return {dq, dk, dv};
 }
@@ -502,8 +456,10 @@ Tensor layernorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& gamma, con
   a.dbeta = dbeta.data_ptr<float>();
   a.rows = (int)(x.numel() / H);
   a.H = H;
+  Tensor ws = torch::empty({(int64_t)ab_layernorm_bwd_slots(a.rows, H), 2, H}, x.options().dtype(at::kFloat));
+  a.ws = ws.data_ptr<float>();
   AB_CHECK_RC(ab_layernorm_bwd(&a, cur_stream()), "ab_layernorm_bwd");
-  g_launches += 1;
+  g_launches += 3;   // row kernel + fixed-order reductions of dgamma and dbeta
   return dx;
 }
 
@@ -557,9 +513,13 @@ Tensor embedding_fwd(const Tensor& ids, const OptTensor& pos, const Tensor& wte,
 
 void embedding_bwd_(const Tensor& ids, const Tensor& dy, Tensor dtable, int64_t vocab_start) {
   TORCH_CHECK(dtable.scalar_type() == at::kFloat && dtable.is_contiguous() && dy.is_contiguous());
+  TORCH_CHECK(ids.scalar_type() == at::kLong, "embedding_bwd: int64 ids");
   c10::cuda::CUDAGuard guard(dy.device());
-  AB_CHECK_RC(ab_embedding_bwd(ids.data_ptr<int64_t>(), bf16_ptr(dy), dtable.data_ptr<float>(),
-                               (int)ids.numel(), (int)dtable.size(1), (int)vocab_start,
+  // a stable sort groups equal ids in token order: the kernel sums each group without atomics (deterministic)
+  auto sorted = at::sort(ids.reshape({-1}), /*stable=*/true, /*dim=*/0, /*descending=*/false);
+  Tensor sorted_ids = std::get<0>(sorted).contiguous(), order = std::get<1>(sorted).contiguous();
+  AB_CHECK_RC(ab_embedding_bwd(sorted_ids.data_ptr<int64_t>(), order.data_ptr<int64_t>(), bf16_ptr(dy),
+                               dtable.data_ptr<float>(), (int)ids.numel(), (int)dtable.size(1), (int)vocab_start,
                                (int)dtable.size(0), cur_stream()),
               "ab_embedding_bwd");
   g_launches += 1;
@@ -568,10 +528,12 @@ void embedding_bwd_(const Tensor& ids, const Tensor& dy, Tensor dtable, int64_t 
 void colsum_(const Tensor& x, Tensor out) {
   TORCH_CHECK(x.dim() == 2 && x.stride(1) == 1 && out.scalar_type() == at::kFloat);
   c10::cuda::CUDAGuard guard(x.device());
-  AB_CHECK_RC(ab_colsum(bf16_ptr(x), out.data_ptr<float>(), (int)x.size(0), (int)x.size(1),
-                        x.stride(0), cur_stream()),
+  const int M = (int)x.size(0), N = (int)x.size(1);
+  if (M == 0) return;
+  Tensor ws = torch::empty({(int64_t)ab_colsum_slots(M, N), N}, x.options().dtype(at::kFloat));
+  AB_CHECK_RC(ab_colsum(bf16_ptr(x), out.data_ptr<float>(), ws.data_ptr<float>(), M, N, x.stride(0), cur_stream()),
               "ab_colsum");
-  g_launches += 1;
+  g_launches += 2;   // partials + fixed-order reduction
 }
 
 // Builds the device-side tensor/chunk tables for the fused optimizer. Returns (tensors, chunks).
@@ -632,11 +594,12 @@ Tensor grad_sumsq(const Tensor& tensors, const Tensor& chunks) {
   c10::cuda::CUDAGuard guard(tensors.device());
   Tensor out = torch::zeros({1}, tensors.options().dtype(at::kFloat));
   const int nchunks = (int)(chunks.numel() / sizeof(ab::AdamChunk));
+  Tensor ws = torch::empty({(int64_t)std::max(1, ab_sumsq_slots(nchunks))}, tensors.options().dtype(at::kFloat));
   AB_CHECK_RC(ab_sumsq(reinterpret_cast<const ab::AdamTensor*>(tensors.data_ptr()),
                        reinterpret_cast<const ab::AdamChunk*>(chunks.data_ptr()), nchunks,
-                       out.data_ptr<float>(), cur_stream()),
+                       out.data_ptr<float>(), ws.data_ptr<float>(), cur_stream()),
               "ab_sumsq");
-  g_launches += 1;
+  g_launches += 2;   // partials + fixed-order reduction
   return out;
 }
 
@@ -741,7 +704,7 @@ Tensor gemm_fp8(const Tensor& x, const Tensor& w, const Tensor& w_scale, const O
   return out;
 }
 
-// Cross-mesh resharding pack / unpack (pack_sm100.cu): `views` are <= 4-D slices with a contiguous innermost dim; tile k
+// Cross-mesh resharding pack / unpack (pack_sm90.cu): `views` are <= 4-D slices with a contiguous innermost dim; tile k
 // lives in `flat` (uint8) at the 16-byte aligned running offset.  unpack = false: views -> flat; true: flat -> views.
 void pack_tiles(const std::vector<Tensor>& views, Tensor flat, bool unpack) {
   TORCH_CHECK(flat.is_cuda() && flat.scalar_type() == at::kByte && flat.is_contiguous(), "pack_tiles: flat must be uint8");
@@ -777,8 +740,8 @@ void pack_tiles(const std::vector<Tensor>& views, Tensor flat, bool unpack) {
   }
 }
 
-// Block-scaled MXFP8: e4m3 elements + one UE8M0 scale per 32 K elements, scale atoms in the tcgen05 layout
-// (gemm_mxfp8_sm100.cu).  Returns (q [M, K] e4m3, sf uint8 [ceil(M/128), ceil(K/128), 512]).
+// Block-scaled MXFP8: e4m3 elements + one UE8M0 scale per 32 K elements, scale atoms of 128 rows x 4 K-blocks
+// (gemm_sm90.cu).  Returns (q [M, K] e4m3, sf uint8 [ceil(M/128), ceil(K/128), 512]).
 std::vector<Tensor> quantize_mxfp8(const Tensor& x) {
   TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.stride(1) == 1, "quantize_mxfp8: x");
   c10::cuda::CUDAGuard guard(x.device());
@@ -892,7 +855,7 @@ Tensor decode_attention(const Tensor& q, const Tensor& k_new, const Tensor& v_ne
   a.o = reinterpret_cast<__nv_bfloat16*>(o.data_ptr());
   // split the key range so that ~2 CTAs per SM stream the cache (the length is only known on the device)
   const int bh = a.B * a.heads;
-  a.splits = std::max(1, std::min(16, (2 * 148 + bh - 1) / bh));
+  a.splits = std::max(1, std::min(16, (2 * ab::num_sms() + bh - 1) / bh));
   Tensor ws;
   if (a.splits > 1) {
     // arrival counters: one persistent zeroed buffer per device; the merging CTA resets its counter
@@ -911,7 +874,7 @@ Tensor decode_attention(const Tensor& q, const Tensor& k_new, const Tensor& v_ne
 }
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "alpa_b200 sm_100a kernels";
+  m.doc() = "alpa_b200 sm_90a kernels";
   m.def("launch_count", []() { return (long long)g_launches.load(); });
   // kernels replayed from a captured CUDA graph are launched by the driver, not through these bindings: the executor
   // adds the number it recorded at capture time for every replay
@@ -928,14 +891,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("ag_push", &ag_push);
   m.def("gemm_wait_a", &gemm_wait_a);
   m.def("allreduce_multimem", &allreduce_multimem, py::arg("mc_ptr"), py::arg("numel"), py::arg("rank"), py::arg("tp"),
-        py::arg("ctas") = 148);
+        py::arg("ctas") = 0);
   m.def("peer_barrier", &peer_barrier);
   m.def("peer_barrier_auto", &peer_barrier_auto);
   m.def("allreduce_oneshot", &allreduce_oneshot, py::arg("x"), py::arg("sym_local_ptr"), py::arg("mc_ptr"),
         py::arg("half_stride"), py::arg("out"), py::arg("flag_ptrs"), py::arg("counter"), py::arg("rank"),
         py::arg("residual") = py::none());
   m.def("attention_fwd", &attention_fwd, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("scale"), py::arg("causal"),
-        py::arg("kv_len") = py::none(), py::arg("trace") = py::none());
+        py::arg("kv_len") = py::none());
   m.def("attention_bwd", &attention_bwd, py::arg("d_o"), py::arg("q"), py::arg("k"), py::arg("v"), py::arg("o"),
         py::arg("lse"), py::arg("scale"), py::arg("causal"), py::arg("dq_out") = py::none(),
         py::arg("dk_out") = py::none(), py::arg("dv_out") = py::none());

@@ -1,10 +1,12 @@
-// C interface of the non-GEMM sm_100a kernels (norm_loss_optim.cu, attention_sm100.cu, comm.cu).
+// C interface of the non-GEMM sm_90a kernels (norm_loss_optim.cu, attention_sm90.cu, comm_sm90.cu, ...).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 namespace ab {
+
+int num_sms();  // SMs of the current device (queried once)
 
 struct LayerNormArgs {
   const __nv_bfloat16* x = nullptr;
@@ -29,6 +31,7 @@ struct LayerNormBwdArgs {
   __nv_bfloat16* dx = nullptr;
   float* dgamma = nullptr;  // accumulated (+=)
   float* dbeta = nullptr;   // accumulated (+=)
+  float* ws = nullptr;      // [ab_layernorm_bwd_slots(rows, H)][2][H] scratch: per-CTA partials of dgamma / dbeta
   int rows = 0, H = 0;
 };
 
@@ -64,10 +67,9 @@ struct AttnArgs {
   int causal = 0;
   // optional device-side number of valid keys (<= Skv): lets one captured graph serve every decode position
   const int* kv_len = nullptr;
-  long long* trace = nullptr;   // optional [1024] clock64 timeline of one CTA (third-generation forward; diagnostic)
 };
 
-// Weight-streaming GEMV of the decode step (gemv_decode_sm100.cu): y[M<=8, N] = act(x[M,K] W[N,K]^T * scale + bias) + res
+// Weight-streaming GEMV of the decode step (gemv_decode_sm90.cu): y[M<=8, N] = act(x[M,K] W[N,K]^T * scale + bias) + res
 struct GemvArgs {
   const __nv_bfloat16* x = nullptr;
   const void* w = nullptr;               // [N, K] e4m3 (fp8 = 1) or bf16
@@ -86,17 +88,15 @@ struct GemvArgs {
 struct AttnBwdArgs {
   AttnArgs f;                          // q,k,v,o,lse + shapes/strides/scale/causal of the forward
   const __nv_bfloat16* d_o = nullptr;  // [B,S,h,D], same strides as o
-  float* dq_accum = nullptr;           // [B,heads,Sq,D] fp32, zero-initialised by the caller
   __nv_bfloat16* dk = nullptr;         // [B,Skv,heads,D] contiguous
   __nv_bfloat16* dv = nullptr;
-  float* delta = nullptr;              // [B,heads,Sq] scratch: rowsum(dO * O)   (split kernels: its negation)
-  float* nlse2 = nullptr;              // [B,heads,Sq] scratch of the split kernels: -lse * log2(e)
+  float* delta = nullptr;              // [B,heads,Sq] scratch: rowsum(dO * O)
   // output strides in elements (b, s, h); D contiguous.  Lets dq/dk/dv be views of one packed
   // [B,S,h,3,D] gradient buffer so the fused-QKV dgrad/wgrad GEMMs read it without a copy.
   long long dq_stride_b = 0, dq_stride_s = 0, dq_stride_h = 0;
   long long dk_stride_b = 0, dk_stride_s = 0, dk_stride_h = 0;
   long long dv_stride_b = 0, dv_stride_s = 0, dv_stride_h = 0;
-  __nv_bfloat16* dq = nullptr;         // bf16 result of the dq_accum conversion
+  __nv_bfloat16* dq = nullptr;
 };
 
 // Ragged 1-D token batch over a slot-addressed KV cache (serving with iteration-level batching).
@@ -113,7 +113,7 @@ struct RaggedAttnArgs {
   float scale = 1.f;
 };
 
-// Decode-step attention with fused KV-cache append (decode_attention_sm100.cu)
+// Decode-step attention with fused KV-cache append (decode_attention_sm90.cu)
 struct DecodeAttnArgs {
   const __nv_bfloat16* q = nullptr;        // [B, heads, D] view, D contiguous
   const __nv_bfloat16* k_new = nullptr;    // [B, heads, D] views with one stride pair
@@ -129,7 +129,7 @@ struct DecodeAttnArgs {
   float scale = 1.f;
 };
 
-// Sharding-invariant counter-based dropout (dropout_sm100.cu)
+// Sharding-invariant counter-based dropout (dropout_sm90.cu)
 constexpr int kDropoutMaxDims = 6;
 struct DropoutArgs {
   const void* x = nullptr;
@@ -155,7 +155,7 @@ struct MoePeers {
 };
 }  // namespace ab
 
-// ---- cross-mesh resharding pack / unpack (pack_sm100.cu)
+// ---- cross-mesh resharding pack / unpack (pack_sm90.cu)
 namespace ab {
 constexpr int kMaxPackTiles = 32;
 struct PackTile {
@@ -172,13 +172,9 @@ struct PackArgs {
 }  // namespace ab
 
 extern "C" {
-int ab_attention_fwd(const ab::AttnArgs* a, cudaStream_t st);
-int ab_attention_fwd2(const ab::AttnArgs* a, cudaStream_t st);      // 16 softmax warps, per-group accumulators
-int ab_attention_fwd3(const ab::AttnArgs* a, cudaStream_t st);      // two softmax warp sets on alternating key tiles
-int ab_attention_fwd4(const ab::AttnArgs* a, cudaStream_t st);      // persistent CTAs on top of the two-set design
+int ab_attention_fwd(const ab::AttnArgs* a, int wide, cudaStream_t st);  // wide: 128-query tiles, else 64
 int ab_attention_bwd(const ab::AttnBwdArgs* a, cudaStream_t st);
 int ab_gemv_decode(const ab::GemvArgs* a, cudaStream_t st);
-int ab_attention_bwd2(const ab::AttnBwdArgs* a, cudaStream_t st);   // split dK/dV + dQ kernels (no atomics)
 int ab_ragged_attention(const ab::RaggedAttnArgs* a, cudaStream_t st);
 int ab_decode_attention(const ab::DecodeAttnArgs* a, cudaStream_t st);
 int ab_dropout(const ab::DropoutArgs* a, int is_bf16, cudaStream_t st);
@@ -195,6 +191,7 @@ int ab_allreduce_oneshot(const __nv_bfloat16* x, __nv_bfloat16* sym_local, const
 int ab_peer_barrier_auto(uint32_t* const* peer_flags, uint32_t* counter, int rank, int tp, cudaStream_t st);
 int ab_layernorm_fwd(const ab::LayerNormArgs* a, cudaStream_t st);
 int ab_layernorm_bwd(const ab::LayerNormBwdArgs* a, cudaStream_t st);
+int ab_layernorm_bwd_slots(int rows, int H);
 int ab_ce_stats(const __nv_bfloat16* logits, const int64_t* labels, float* stats, int rows, int V,
                 int vocab_start, long long ld, cudaStream_t st);
 int ab_ce_grad(__nv_bfloat16* logits, const int64_t* labels, const float* gstats,
@@ -203,9 +200,12 @@ int ab_ce_grad(__nv_bfloat16* logits, const int64_t* labels, const float* gstats
 int ab_embedding_fwd(const int64_t* ids, const int64_t* pos, const __nv_bfloat16* wte,
                      const __nv_bfloat16* wpe, __nv_bfloat16* out, int T, int H, int vocab_start,
                      int Vlocal, cudaStream_t st);
-int ab_embedding_bwd(const int64_t* ids, const __nv_bfloat16* dy, float* dtable, int T, int H,
-                     int vocab_start, int Vlocal, cudaStream_t st);
-int ab_colsum(const __nv_bfloat16* x, float* out, int M, int N, long long ld, cudaStream_t st);
+// sorted_ids / order: the token ids sorted stably by value and the token index at each sorted position
+int ab_embedding_bwd(const int64_t* sorted_ids, const int64_t* order, const __nv_bfloat16* dy, float* dtable, int T,
+                     int H, int vocab_start, int Vlocal, cudaStream_t st);
+// ws: [ab_colsum_slots(M, N)][N] fp32 scratch
+int ab_colsum_slots(int M, int N);
+int ab_colsum(const __nv_bfloat16* x, float* out, float* ws, int M, int N, long long ld, cudaStream_t st);
 int ab_adamw(const ab::AdamTensor* tensors, const ab::AdamChunk* chunks, int num_chunks, float lr,
              float beta1, float beta2, float eps, float bc1, float bc2, float grad_scale,
              const float* clip_coef, const float* step_ptr, cudaStream_t st);
@@ -227,6 +227,8 @@ int ab_pack_tiles(const ab::PackArgs* args, int unpack, cudaStream_t st);
 int ab_quantize_rows_mxfp8(const __nv_bfloat16* x, uint8_t* q, uint8_t* sf, int M, int K, long long ldx, cudaStream_t st);
 int ab_gemm_mxfp8(const uint8_t* a, const uint8_t* sfa, const uint8_t* b, const uint8_t* sfb, const __nv_bfloat16* bias,
                   __nv_bfloat16* out, int M, int N, int K, long long ldc, int act, cudaStream_t st);
-int ab_sumsq(const ab::AdamTensor* tensors, const ab::AdamChunk* chunks, int num_chunks, float* out,
+// ws: [ab_sumsq_slots(num_chunks)] fp32 scratch
+int ab_sumsq_slots(int num_chunks);
+int ab_sumsq(const ab::AdamTensor* tensors, const ab::AdamChunk* chunks, int num_chunks, float* out, float* ws,
              cudaStream_t st);
 }

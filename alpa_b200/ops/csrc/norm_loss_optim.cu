@@ -1,4 +1,4 @@
-// Bandwidth-bound sm_100a kernels: LayerNorm fwd/bwd (fused residual add), vocab-parallel softmax
+// Bandwidth-bound sm_90a kernels: LayerNorm fwd/bwd (fused residual add), vocab-parallel softmax
 // cross-entropy (stats + in-place gradient), embedding gather / scatter-add, column sum (bias grad),
 // fused multi-tensor AdamW on fp32 master weights, grad-norm, bf16<->fp32 casts.
 //
@@ -139,8 +139,7 @@ __global__ void __launch_bounds__(kLnThreads)
 layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
                      const __nv_bfloat16* __restrict__ gamma, const float* __restrict__ mean,
                      const float* __restrict__ rstd, const __nv_bfloat16* __restrict__ dres,
-                     __nv_bfloat16* __restrict__ dx, float* __restrict__ dgamma,
-                     float* __restrict__ dbeta, int rows, int H) {
+                     __nv_bfloat16* __restrict__ dx, float* __restrict__ ws, int rows, int H) {
   __shared__ float sh[32];
   const int nvec = H / 8;
   float ag[kChunks][8], abt[kChunks][8];
@@ -215,9 +214,9 @@ layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* 
     const int vi = threadIdx.x + c * kLnThreads;
     if (vi < nvec) {
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        atomicAdd(dgamma + vi * 8 + j, ag[c][j]);
-        atomicAdd(dbeta + vi * 8 + j, abt[c][j]);
+      for (int j = 0; j < 8; ++j) {  // this CTA's partial sums (reduced in a fixed order by reduce_slots_kernel)
+        ws[(size_t)blockIdx.x * 2 * H + vi * 8 + j] = ag[c][j];
+        ws[(size_t)blockIdx.x * 2 * H + H + vi * 8 + j] = abt[c][j];
       }
     }
   }
@@ -334,15 +333,10 @@ __global__ void __launch_bounds__(256)
 layernorm_bwd_warp_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
                           const __nv_bfloat16* __restrict__ gamma, const float* __restrict__ mean,
                           const float* __restrict__ rstd, const __nv_bfloat16* __restrict__ dres,
-                          __nv_bfloat16* __restrict__ dx, float* __restrict__ dgamma, float* __restrict__ dbeta,
-                          int rows) {
+                          __nv_bfloat16* __restrict__ dx, float* __restrict__ ws, int rows) {
   constexpr int H = VPL * WPR * 256;
-  extern __shared__ float sh_gb[];   // [2][H]
+  extern __shared__ float sh_gb[];   // [row groups][2][H]
   __shared__ float2 xch[16][WPR];
-  float* sh_g = sh_gb;
-  float* sh_b = sh_gb + H;
-  for (int i = threadIdx.x; i < 2 * H; i += blockDim.x) sh_gb[i] = 0.f;
-  __syncthreads();
   const int lane = threadIdx.x & 31;
   const int wib = threadIdx.x >> 5;
   const int grp = wib / WPR, wr = wib % WPR;
@@ -407,20 +401,33 @@ layernorm_bwd_warp_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloa
       *reinterpret_cast<int4*>(dx + (size_t)row * H + off) = o;
     }
   }
-  // CTA-level reduction of the per-lane partials, then one global atomic per column per CTA
+  // CTA-level reduction of the per-lane partials in a fixed order (row group 0, 1, ...): every column has exactly one
+  // owner lane per row group; the CTA's sums go to ws[blockIdx.x] and are reduced over CTAs by reduce_slots_kernel
 #pragma unroll
   for (int c = 0; c < VPL; ++c)
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const int col = ((c * WPR + wr) * 32 + lane) * 8 + j;
-      atomicAdd(&sh_g[col], ag[c][j]);
-      atomicAdd(&sh_b[col], ab[c][j]);
+      sh_gb[grp * 2 * H + col] = ag[c][j];
+      sh_gb[grp * 2 * H + H + col] = ab[c][j];
     }
   __syncthreads();
-  for (int i = threadIdx.x; i < H; i += blockDim.x) {
-    atomicAdd(dgamma + i, sh_g[i]);
-    atomicAdd(dbeta + i, sh_b[i]);
+  for (int i = threadIdx.x; i < 2 * H; i += blockDim.x) {
+    float t = 0.f;
+    for (int g = 0; g < groups_per_cta; ++g) t += sh_gb[g * 2 * H + i];
+    ws[(size_t)blockIdx.x * 2 * H + i] = t;
   }
+}
+
+// out[c] += sum over s = 0, 1, ... of ws[s * ld + c]: the fixed-order second pass of every cross-CTA reduction below,
+// so results do not depend on which CTA finishes first.
+__global__ void __launch_bounds__(256)
+reduce_slots_kernel(const float* __restrict__ ws, int slots, long long ld, int n, float* __restrict__ out) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n) return;
+  float t = 0.f;
+  for (int s = 0; s < slots; ++s) t += ws[(size_t)s * ld + c];
+  out[c] += t;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -527,16 +534,29 @@ __global__ void embedding_fwd_kernel(const int64_t* __restrict__ ids, const int6
   }
 }
 
-__global__ void embedding_bwd_kernel(const int64_t* __restrict__ ids, const __nv_bfloat16* __restrict__ dy,
-                                     float* __restrict__ dtable, int T, int H, int vocab_start,
-                                     int Vlocal) {
-  for (int t = blockIdx.x; t < T; t += gridDim.x) {
-    const long long id = ids[t] - vocab_start;
+// sorted_ids / order: the token ids sorted stably and the token index of each sorted position.  The CTA at the first
+// position of a run of equal ids sums that run's rows in token order and adds the result once: no atomics, so the
+// gradient does not depend on scheduling.
+__global__ void embedding_bwd_kernel(const int64_t* __restrict__ sorted_ids, const int64_t* __restrict__ order,
+                                     const __nv_bfloat16* __restrict__ dy, float* __restrict__ dtable, int T, int H,
+                                     int vocab_start, int Vlocal) {
+  for (int i = blockIdx.x; i < T; i += gridDim.x) {
+    const long long raw = sorted_ids[i];
+    if (i > 0 && sorted_ids[i - 1] == raw) continue;
+    const long long id = raw - vocab_start;
     if (id < 0 || id >= Vlocal) continue;
+    int end = i + 1;
+    while (end < T && sorted_ids[end] == raw) ++end;
     for (int c = threadIdx.x; c < H / 2; c += blockDim.x) {
-      const float2 f = unpack_bf16x2(reinterpret_cast<const uint32_t*>(dy + (size_t)t * H)[c]);
-      atomicAdd(dtable + (size_t)id * H + 2 * c, f.x);
-      atomicAdd(dtable + (size_t)id * H + 2 * c + 1, f.y);
+      float sx = 0.f, sy = 0.f;
+      for (int j = i; j < end; ++j) {
+        const float2 f = unpack_bf16x2(reinterpret_cast<const uint32_t*>(dy + (size_t)order[j] * H)[c]);
+        sx += f.x;
+        sy += f.y;
+      }
+      float2* o = reinterpret_cast<float2*>(dtable + (size_t)id * H) + c;
+      const float2 old = *o;
+      *o = make_float2(old.x + sx, old.y + sy);
     }
   }
 }
@@ -546,7 +566,7 @@ __global__ void embedding_bwd_kernel(const int64_t* __restrict__ ids, const __nv
 // ------------------------------------------------------------------------------------------------
 // block = (32 column groups of 8) x (8 row lanes); 4 rows x 16 bytes in flight per thread
 __global__ void __launch_bounds__(256)
-colsum_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ out, int M, int N, long long ld,
+colsum_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ ws, int M, int N, long long ld,
               int rows_per_block) {
   __shared__ float red[8][256 + 8];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
@@ -590,7 +610,7 @@ colsum_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ out, int 
     float t = 0.f;
 #pragma unroll
     for (int y = 0; y < 8; ++y) t += red[y][c];
-    atomicAdd(out + blockIdx.x * 256 + c, t);
+    ws[(size_t)blockIdx.y * N + blockIdx.x * 256 + c] = t;   // row block y's partial
   }
 }
 
@@ -673,7 +693,7 @@ adamw_kernel(const AdamTensor* __restrict__ tensors, const AdamChunk* __restrict
 // sum of squares over a table of tensors -> out[0] (fp32), for global-norm clipping.
 __global__ void __launch_bounds__(256)
 sumsq_kernel(const AdamTensor* __restrict__ tensors, const AdamChunk* __restrict__ chunks,
-             int num_chunks, float* __restrict__ out) {
+             int num_chunks, float* __restrict__ ws) {
   __shared__ float sh[32];
   float s = 0.f;
   for (int ci = blockIdx.x; ci < num_chunks; ci += gridDim.x) {
@@ -687,7 +707,7 @@ sumsq_kernel(const AdamTensor* __restrict__ tensors, const AdamChunk* __restrict
     }
   }
   s = block_sum<256>(s, sh);
-  if (threadIdx.x == 0) atomicAdd(out, s);
+  if (threadIdx.x == 0) ws[blockIdx.x] = s;
 }
 
 }  // namespace ab
@@ -702,17 +722,28 @@ static void ln_fwd_launch(const LayerNormArgs& a, cudaStream_t st, int grid) {
 template <int kChunks>
 static void ln_bwd_launch(const LayerNormBwdArgs& a, cudaStream_t st, int grid) {
   layernorm_bwd_kernel<kChunks><<<grid, kLnThreads, 0, st>>>(
-      a.dy, a.x, a.gamma, a.mean, a.rstd, a.dres, a.dx, a.dgamma, a.dbeta, a.rows, a.H);
+      a.dy, a.x, a.gamma, a.mean, a.rstd, a.dres, a.dx, a.ws, a.rows, a.H);
+}
+static int ln_bwd_generic_grid(int rows) { return rows < ab::num_sms() * 2 ? rows : ab::num_sms() * 2; }
+template <int WPR>
+static int ln_bwd_warp_grid(int rows) {
+  const int gpc = 8 / WPR;
+  int grid = (rows + gpc - 1) / gpc;
+  if (grid > ab::num_sms() * 2) {
+    const int iters = (rows + ab::num_sms() * 2 * gpc - 1) / (ab::num_sms() * 2 * gpc);
+    grid = (rows + iters * gpc - 1) / (iters * gpc);
+  }
+  return grid;
 }
 
 template <int VPL, int WPR>
 static void ln_fwd_warp_launch(const LayerNormArgs& a, cudaStream_t st) {
   const int gpc = 8 / WPR;
   int grid = (a.rows + gpc - 1) / gpc;
-  if (grid > 148 * 8) {
+  if (grid > ab::num_sms() * 8) {
     // balanced persistent grid: every row group runs the same number of rows (16384 rows on 1184 CTAs would leave a
     // 27 % idle tail: some groups get 2 rows, most of the second wave only 1)
-    const int iters = (a.rows + 148 * 8 * gpc - 1) / (148 * 8 * gpc);
+    const int iters = (a.rows + ab::num_sms() * 8 * gpc - 1) / (ab::num_sms() * 8 * gpc);
     grid = (a.rows + iters * gpc - 1) / (iters * gpc);
   }
   layernorm_fwd_warp_kernel<VPL, WPR><<<grid, 256, 0, st>>>(a.x, a.residual, a.gamma, a.beta, a.y, a.sum_out,
@@ -722,19 +753,15 @@ template <int VPL, int WPR>
 static void ln_bwd_warp_launch(const LayerNormBwdArgs& a, cudaStream_t st) {
   const int gpc = 8 / WPR;
   constexpr int H = VPL * WPR * 256;
-  int grid = (a.rows + gpc - 1) / gpc;
-  if (grid > 148 * 2) {
-    const int iters = (a.rows + 148 * 2 * gpc - 1) / (148 * 2 * gpc);
-    grid = (a.rows + iters * gpc - 1) / (iters * gpc);
-  }
+  const int grid = ln_bwd_warp_grid<WPR>(a.rows);
+  const int smem = gpc * 2 * H * (int)sizeof(float);
   static bool attr_set = false;
   if (!attr_set) {
-    cudaFuncSetAttribute(layernorm_bwd_warp_kernel<VPL, WPR>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         2 * H * (int)sizeof(float));
+    cudaFuncSetAttribute(layernorm_bwd_warp_kernel<VPL, WPR>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     attr_set = true;
   }
-  layernorm_bwd_warp_kernel<VPL, WPR><<<grid, 256, 2 * H * sizeof(float), st>>>(
-      a.dy, a.x, a.gamma, a.mean, a.rstd, a.dres, a.dx, a.dgamma, a.dbeta, a.rows);
+  layernorm_bwd_warp_kernel<VPL, WPR><<<grid, 256, smem, st>>>(
+      a.dy, a.x, a.gamma, a.mean, a.rstd, a.dres, a.dx, a.ws, a.rows);
 }
 
 extern "C" int ab_layernorm_fwd(const LayerNormArgs* a, cudaStream_t st) {
@@ -760,39 +787,60 @@ extern "C" int ab_layernorm_fwd(const LayerNormArgs* a, cudaStream_t st) {
   }
 generic_fwd:
   const int chunks = (a->H / 8 + kLnThreads - 1) / kLnThreads;
-  const int grid = a->rows < 148 * 8 ? a->rows : 148 * 8;
+  const int grid = a->rows < ab::num_sms() * 8 ? a->rows : ab::num_sms() * 8;
   if (chunks <= 1) ln_fwd_launch<1>(*a, st, grid);
   else if (chunks <= 2) ln_fwd_launch<2>(*a, st, grid);
   else if (chunks <= 4) ln_fwd_launch<4>(*a, st, grid);
   else ln_fwd_launch<8>(*a, st, grid);
   return cudaGetLastError() == cudaSuccess ? 0 : 2;
 }
-extern "C" int ab_layernorm_bwd(const LayerNormBwdArgs* a, cudaStream_t st) {
-  if (a->H % 8 != 0 || a->H > kLnThreads * 8 * 4) return 1;
-  if (a->H % 256 == 0 && a->H <= 8192) {
-    switch (a->H / 256) {
-      case 1: ln_bwd_warp_launch<1, 1>(*a, st); break;
-      case 2: ln_bwd_warp_launch<2, 1>(*a, st); break;
-      case 3: ln_bwd_warp_launch<3, 1>(*a, st); break;
-      case 4: ln_bwd_warp_launch<4, 1>(*a, st); break;
-      case 6: ln_bwd_warp_launch<3, 2>(*a, st); break;
-      case 8: ln_bwd_warp_launch<4, 2>(*a, st); break;
-      case 10: ln_bwd_warp_launch<5, 2>(*a, st); break;
-      case 12: ln_bwd_warp_launch<3, 4>(*a, st); break;
-      case 16: ln_bwd_warp_launch<4, 4>(*a, st); break;
-      case 20: ln_bwd_warp_launch<5, 4>(*a, st); break;
-      case 24: ln_bwd_warp_launch<3, 8>(*a, st); break;
-      case 32: ln_bwd_warp_launch<4, 8>(*a, st); break;
-      default: goto generic_bwd;
-    }
-    return cudaGetLastError() == cudaSuccess ? 0 : 2;
+// (VPL, WPR) of the warp-group kernel for H, or 0 when the generic kernel runs
+static int ln_bwd_warp_cfg(int H) {
+  if (H % 256 != 0 || H > 8192) return 0;
+  switch (H / 256) {
+    case 1: return 11; case 2: return 21; case 3: return 31; case 4: return 41; case 6: return 32; case 8: return 42;
+    case 10: return 52; case 12: return 34; case 16: return 44; case 20: return 54; case 24: return 38; case 32: return 48;
   }
-generic_bwd:
-  const int chunks = (a->H / 8 + kLnThreads - 1) / kLnThreads;
-  const int grid = a->rows < 148 * 2 ? a->rows : 148 * 2;
-  if (chunks <= 1) ln_bwd_launch<1>(*a, st, grid);
-  else if (chunks <= 2) ln_bwd_launch<2>(*a, st, grid);
-  else ln_bwd_launch<4>(*a, st, grid);
+  return 0;
+}
+// Number of per-CTA partial rows ([2][H] floats each) ab_layernorm_bwd writes into a.ws.
+extern "C" int ab_layernorm_bwd_slots(int rows, int H) {
+  const int cfg = ln_bwd_warp_cfg(H);
+  if (cfg == 0) return ln_bwd_generic_grid(rows);
+  switch (cfg % 10) {
+    case 1: return ln_bwd_warp_grid<1>(rows);
+    case 2: return ln_bwd_warp_grid<2>(rows);
+    case 4: return ln_bwd_warp_grid<4>(rows);
+    default: return ln_bwd_warp_grid<8>(rows);
+  }
+}
+extern "C" int ab_layernorm_bwd(const LayerNormBwdArgs* a, cudaStream_t st) {
+  if (a->H % 8 != 0 || a->H > kLnThreads * 8 * 4 || a->ws == nullptr) return 1;
+  switch (ln_bwd_warp_cfg(a->H)) {
+    case 11: ln_bwd_warp_launch<1, 1>(*a, st); break;
+    case 21: ln_bwd_warp_launch<2, 1>(*a, st); break;
+    case 31: ln_bwd_warp_launch<3, 1>(*a, st); break;
+    case 41: ln_bwd_warp_launch<4, 1>(*a, st); break;
+    case 32: ln_bwd_warp_launch<3, 2>(*a, st); break;
+    case 42: ln_bwd_warp_launch<4, 2>(*a, st); break;
+    case 52: ln_bwd_warp_launch<5, 2>(*a, st); break;
+    case 34: ln_bwd_warp_launch<3, 4>(*a, st); break;
+    case 44: ln_bwd_warp_launch<4, 4>(*a, st); break;
+    case 54: ln_bwd_warp_launch<5, 4>(*a, st); break;
+    case 38: ln_bwd_warp_launch<3, 8>(*a, st); break;
+    case 48: ln_bwd_warp_launch<4, 8>(*a, st); break;
+    default: {
+      const int chunks = (a->H / 8 + kLnThreads - 1) / kLnThreads;
+      const int grid = ln_bwd_generic_grid(a->rows);
+      if (chunks <= 1) ln_bwd_launch<1>(*a, st, grid);
+      else if (chunks <= 2) ln_bwd_launch<2>(*a, st, grid);
+      else ln_bwd_launch<4>(*a, st, grid);
+    }
+  }
+  const int slots = ab_layernorm_bwd_slots(a->rows, a->H);
+  const int blocks = (a->H + 255) / 256;
+  reduce_slots_kernel<<<blocks, 256, 0, st>>>(a->ws, slots, 2LL * a->H, a->H, a->dgamma);
+  reduce_slots_kernel<<<blocks, 256, 0, st>>>(a->ws + a->H, slots, 2LL * a->H, a->H, a->dbeta);
   return cudaGetLastError() == cudaSuccess ? 0 : 2;
 }
 extern "C" int ab_ce_stats(const __nv_bfloat16* logits, const int64_t* labels, float* stats, int rows,
@@ -812,42 +860,54 @@ extern "C" int ab_embedding_fwd(const int64_t* ids, const int64_t* pos, const __
                                 const __nv_bfloat16* wpe, __nv_bfloat16* out, int T, int H,
                                 int vocab_start, int Vlocal, cudaStream_t st) {
   if (H % 8 != 0) return 1;
-  const int grid = T < 148 * 16 ? T : 148 * 16;
+  const int grid = T < ab::num_sms() * 16 ? T : ab::num_sms() * 16;
   embedding_fwd_kernel<<<grid, 128, 0, st>>>(ids, pos, wte, wpe, out, T, H, vocab_start, Vlocal);
   return cudaGetLastError() == cudaSuccess ? 0 : 2;
 }
-extern "C" int ab_embedding_bwd(const int64_t* ids, const __nv_bfloat16* dy, float* dtable, int T,
-                                int H, int vocab_start, int Vlocal, cudaStream_t st) {
+extern "C" int ab_embedding_bwd(const int64_t* sorted_ids, const int64_t* order, const __nv_bfloat16* dy,
+                                float* dtable, int T, int H, int vocab_start, int Vlocal, cudaStream_t st) {
   if (H % 2 != 0) return 1;
-  const int grid = T < 148 * 16 ? T : 148 * 16;
-  embedding_bwd_kernel<<<grid, 256, 0, st>>>(ids, dy, dtable, T, H, vocab_start, Vlocal);
+  const int grid = T < ab::num_sms() * 16 ? T : ab::num_sms() * 16;
+  embedding_bwd_kernel<<<grid, 256, 0, st>>>(sorted_ids, order, dy, dtable, T, H, vocab_start, Vlocal);
   return cudaGetLastError() == cudaSuccess ? 0 : 2;
 }
-extern "C" int ab_colsum(const __nv_bfloat16* x, float* out, int M, int N, long long ld,
-                         cudaStream_t st) {
-  if (N % 8 != 0 || ld % 8 != 0 || (reinterpret_cast<uintptr_t>(x) & 15) != 0) return 1;
+// row blocks of the column sum (partials written to ws[gy][N])
+static int colsum_rows_per_block(int M, int N) {
   const int gx = (N + 255) / 256;
-  int gy = (148 * 8 + gx - 1) / gx;
+  int gy = (ab::num_sms() * 8 + gx - 1) / gx;
   if (gy > (M + 31) / 32) gy = (M + 31) / 32;
   if (gy < 1) gy = 1;
-  const int rpb = (M + gy - 1) / gy;
-  gy = (M + rpb - 1) / rpb;
-  colsum_kernel<<<dim3(gx, gy), 256, 0, st>>>(x, out, M, N, ld, rpb);
+  return (M + gy - 1) / gy;
+}
+extern "C" int ab_colsum_slots(int M, int N) {
+  const int rpb = colsum_rows_per_block(M, N);
+  return (M + rpb - 1) / rpb;
+}
+extern "C" int ab_colsum(const __nv_bfloat16* x, float* out, float* ws, int M, int N, long long ld,
+                         cudaStream_t st) {
+  if (N % 8 != 0 || ld % 8 != 0 || (reinterpret_cast<uintptr_t>(x) & 15) != 0 || M <= 0) return 1;
+  const int gx = (N + 255) / 256;
+  const int rpb = colsum_rows_per_block(M, N);
+  const int gy = ab_colsum_slots(M, N);
+  colsum_kernel<<<dim3(gx, gy), 256, 0, st>>>(x, ws, M, N, ld, rpb);
+  reduce_slots_kernel<<<gx, 256, 0, st>>>(ws, gy, N, N, out);
   return cudaGetLastError() == cudaSuccess ? 0 : 2;
 }
 extern "C" int ab_adamw(const AdamTensor* tensors, const AdamChunk* chunks, int num_chunks, float lr,
                         float beta1, float beta2, float eps, float bc1, float bc2, float grad_scale,
                         const float* clip_coef, const float* step_ptr, cudaStream_t st) {
   if (num_chunks <= 0) return 0;
-  const int grid = num_chunks < 148 * 8 ? num_chunks : 148 * 8;
+  const int grid = num_chunks < ab::num_sms() * 8 ? num_chunks : ab::num_sms() * 8;
   adamw_kernel<<<grid, 256, 0, st>>>(tensors, chunks, num_chunks, lr, beta1, beta2, eps, bc1, bc2,
                                      grad_scale, clip_coef, step_ptr);
   return cudaGetLastError() == cudaSuccess ? 0 : 2;
 }
-extern "C" int ab_sumsq(const AdamTensor* tensors, const AdamChunk* chunks, int num_chunks, float* out,
+extern "C" int ab_sumsq_slots(int num_chunks) { return num_chunks < ab::num_sms() * 4 ? num_chunks : ab::num_sms() * 4; }
+extern "C" int ab_sumsq(const AdamTensor* tensors, const AdamChunk* chunks, int num_chunks, float* out, float* ws,
                         cudaStream_t st) {
   if (num_chunks <= 0) return 0;
-  const int grid = num_chunks < 148 * 4 ? num_chunks : 148 * 4;
-  sumsq_kernel<<<grid, 256, 0, st>>>(tensors, chunks, num_chunks, out);
+  const int grid = ab_sumsq_slots(num_chunks);
+  sumsq_kernel<<<grid, 256, 0, st>>>(tensors, chunks, num_chunks, ws);
+  reduce_slots_kernel<<<1, 256, 0, st>>>(ws, grid, 1, 1, out);
   return cudaGetLastError() == cudaSuccess ? 0 : 2;
 }

@@ -1,6 +1,5 @@
-// Blackwell (sm_100a) PTX wrappers shared by every alpa_b200 kernel:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld),
-// UMMA shared-memory + instruction descriptors, and peer-memory ld/st/red helpers.
+// Hopper (sm_90a) PTX wrappers shared by every alpa_b200 kernel:
+// mbarrier, TMA (cp.async.bulk.tensor) and peer-memory ld/st/red helpers.
 //
 // Everything here is inline PTX; there is no library dependency.
 #pragma once
@@ -51,8 +50,6 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ uint32_t mbar_try_wait(uint64_t* bar, uint32_t parity) {
-  // (a suspend-time hint -- CUTLASS passes 10 ms -- was measured: attention forward 0.173 -> 0.180 ms, backward
-  // 0.445 -> 0.470 ms; the plain form wakes the waiting softmax warps sooner)
   uint32_t ok;
   asm volatile(
       "{\n\t.reg .pred P;\n\t"
@@ -103,44 +100,6 @@ __device__ __forceinline__ float lds_f32(uint32_t saddr) {
   return v;
 }
 
-// ----------------------------------------------------------------------------------------------
-// Packed fp32x2 math (sm_100: FFMA2 / FADD2 / FMUL2, two fp32 results per issued instruction) and the 3-input max
-// (FMNMX3).  The softmax warps of the attention kernels are issue-bound; these halve their ALU instruction count.
-// A pair lives in one 64-bit register: lo = first element.
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t f2_pack(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ uint64_t f2_pack_bits(uint32_t lo, uint32_t hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(lo), "r"(hi));
-  return r;
-}
-__device__ __forceinline__ void f2_unpack(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t ffma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t fadd2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ uint64_t fmul2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -203,221 +162,26 @@ __device__ __forceinline__ void tma_store_wait() {
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma: shared-memory descriptors and group fences
 // ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(
-                   smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-}
-// ---- CTA-pair (cta_group::2) variants: two SMs of one TPC cooperate on a 256-row tile -----------------------
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;   // clears the CTA-rank bit of a shared::cluster address -> CTA 0
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2cta() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// TMA load into this CTA's smem whose completion bytes are counted on the *leader* CTA's mbarrier
-__device__ __forceinline__ void tma_load_3d_2cta(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int32_t c0,
-                                                 int32_t c1, int32_t c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%3, %4, %5}], [%2];\n" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void umma_f16_ss_2cta(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                 uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// MMA completion -> arrive on the barrier at the same smem offset in both CTAs of the pair
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n" ::"r"(
-          smem_u32(bar)),
-      "h"((uint16_t)3)
-      : "memory");
-}
-// arrive on the leader CTA's copy of `bar` (from either CTA of the pair)
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];\n" ::"r"(smem_u32(bar) & kPeerBitMask)
-               : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; bf16/fp16 inputs, fp32 accumulate.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// A operand from TMEM (used by attention: P stays in tensor memory).
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// fp8 (e4m3/e5m2) inputs, fp32 accumulate, no block scaling.
-__device__ __forceinline__ void umma_f8f6f4_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                               uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Block-scaled fp8: scale factors (UE8M0, one per 32 K-elements) live in TMEM.
-__device__ __forceinline__ void umma_mxf8_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                             uint32_t idesc, uint32_t accumulate,
-                                             uint32_t tmem_sfa, uint32_t tmem_sfb) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n\t}\n" ::
-          "r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(tmem_sfa), "r"(tmem_sfb)
-      : "memory");
-}
-// smem -> TMEM copy of scale factors (32 lanes x 128 bit, replicated to the 4 lane quadrants).
-__device__ __forceinline__ void tmem_cp_32x128b_warpx4(uint32_t tmem_dst, uint64_t smem_desc) {
-  asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;\n" ::"r"(tmem_dst), "l"(smem_desc)
-               : "memory");
-}
-// All prior tcgen05.mma of this thread arrive on `bar` when they retire (implies fence::before).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-// 32 lanes x 32 columns of fp32: thread i of the warp receives row (lane base + i), 32 columns.
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-      "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory");
-}
-
-// ----------------------------------------------------------------------------------------------
-// UMMA descriptors (bit layouts: cute/arch/mma_sm100_desc.hpp)
-// ----------------------------------------------------------------------------------------------
-enum : uint32_t { kMajorK = 0, kMajorMN = 1 };
-enum : uint32_t { kFmtF16 = 0, kFmtBF16 = 1, kFmtTF32 = 2 };
-enum : uint32_t { kFmtE4M3 = 0, kFmtE5M2 = 1 };
-
-// Instruction descriptor for kind::f16 / kind::f8f6f4 (fp32 accumulate).
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t a_fmt, uint32_t b_fmt, uint32_t a_major,
-                                                  uint32_t b_major, uint32_t M, uint32_t N) {
-  return (1u << 4)                 // c_format = F32
-         | (a_fmt << 7) | (b_fmt << 10) | (a_major << 15) | (b_major << 16) |
-         ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-// Block-scaled (mxf8f6f4) variant: scale_format=UE8M0 at bit 23, SF ids at [4,6) / [29,31).
-__host__ __device__ constexpr uint32_t make_idesc_mx(uint32_t a_fmt, uint32_t b_fmt, uint32_t M,
-                                                     uint32_t N, uint32_t a_sf_id,
-                                                     uint32_t b_sf_id) {
-  return (b_sf_id << 4) | (a_fmt << 7) | (b_fmt << 10) | ((N >> 3) << 17) | (1u << 23) |
-         ((M >> 4) << 24) | (a_sf_id << 29);
-}
-
-// Shared-memory matrix descriptor, 128-byte swizzle, Blackwell version bits.
-//   K-major  : rows of 128 B (64 bf16 of K); SBO = 8 rows * 128 B; LBO unused.
+// Shared-memory matrix descriptor for wgmma, 128-byte swizzle.
+//   K-major  : rows of 128 B; SBO = 8 rows * 128 B; LBO unused.
 //   MN-major : atoms of [8 k-rows][128 B of MN]; SBO = 1024 B between 8-row k groups,
 //              LBO = byte distance between successive 64-element MN atoms.
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                         uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;  // version = 1 (sm_100)
-  d |= static_cast<uint64_t>(2) << 61;  // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;  // SWIZZLE_128B
   return d;
 }
-// Non-swizzled (interleaved 8x16B core matrices) descriptor, used for scale-factor tcgen05.cp.
-__device__ __forceinline__ uint64_t make_smem_desc_noswz(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                         uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  return d;
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory");
 }
-
 // ----------------------------------------------------------------------------------------------
 // Memory-ordering + peer (NVLink) access helpers for fused compute+collective kernels
 // ----------------------------------------------------------------------------------------------

@@ -7,19 +7,15 @@
 
 namespace ab {
 
-// rank-N bf16 tensor map with 128-byte swizzle. dims/strides innermost first; strides in ELEMENTS
-// (strides[0] is implicitly 1 and ignored); box in elements.
-int make_tmap_bf16(CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims,
-                   const uint64_t* strides_elems, const uint32_t* box);
-
-// 3-D convenience wrapper used by the GEMM: dims (inner, rows, batch).
+// 3-D bf16 tensor map with 128-byte swizzle used by the GEMM: dims (inner, rows, batch), strides in elements.
 int make_tmap_bf16_3d(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t rows,
                       uint64_t batch, uint64_t row_stride_elems, uint64_t batch_stride_elems,
                       uint32_t box_inner, uint32_t box_rows);
 
-// 2-D fp32 tensor map without swizzle (rows of `inner` floats; out-of-bounds elements read as zero).
-int make_tmap_f32_2d(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t rows, uint64_t row_stride_elems,
-                     uint32_t box_inner, uint32_t box_rows);
+// 4-D bf16 tensor map with 128-byte swizzle: dims (inner, rows, d2, d3), strides of dims 1..3 in elements,
+// box (box_inner, box_rows, 1, 1).  Used by the attention kernels on [B, S, heads, D] views.
+int make_tmap_bf16_4d(CUtensorMap* out, const void* ptr, const uint64_t* dims, const uint64_t* strides_elems,
+                      uint32_t box_inner, uint32_t box_rows);
 
 int num_sms();
 

@@ -2,7 +2,7 @@
 
 See ``alpa_b200/ops/__init__.py`` for the contract.  The reference has no counterpart file: its
 primitives are XLA HLO ops lowered to cuBLAS / LLVM fusions (SURVEY.md §2.5 K1-K9); here they are the
-hand-written sm_100a kernels, and the *same* op names appear in traced graphs, plans and programs.
+hand-written sm_90a kernels, and the *same* op names appear in traced graphs, plans and programs.
 """
 from __future__ import annotations
 
@@ -36,7 +36,7 @@ def _native():
 
 
 def uses_native(*tensors: Tensor) -> bool:
-    """True if the sm_100a kernels serve this call: CUDA + bf16 activations.  On CUDA/bf16 a missing
+    """True if the sm_90a kernels serve this call: CUDA + bf16 activations.  On CUDA/bf16 a missing
     extension is an error (no silent eager fallback) unless ALPA_B200_ALLOW_FALLBACK=1."""
     ts = [t for t in tensors if t is not None]
     if not ts or not all(t.is_cuda for t in ts):
@@ -50,7 +50,7 @@ def uses_native(*tensors: Tensor) -> bool:
         return True
     if ops.allow_fallback():
         return False
-    raise RuntimeError("alpa_b200: CUDA bf16 tensors but the sm_100a extension is not built/loaded "
+    raise RuntimeError("alpa_b200: CUDA bf16 tensors but the sm_90a extension is not built/loaded "
                        "(run `python -m alpa_b200.ops.build`; set ALPA_B200_ALLOW_FALLBACK=1 to use PyTorch)")
 
 
@@ -58,8 +58,8 @@ _FALLBACK_SEEN = set()
 
 
 def library_fallbacks():
-    """Operand layouts for which a primitive fell back to a PyTorch library kernel although the sm_100a extension is
-    loaded (shape / stride / alignment outside the tcgen05 kernel's TMA constraints).  One warning per distinct
+    """Operand layouts for which a primitive fell back to a PyTorch library kernel although the sm_90a extension is
+    loaded (shape / stride / alignment outside the wgmma kernel's TMA constraints).  One warning per distinct
     layout is logged; tests and benchmarks can assert this stays empty."""
     return sorted(_FALLBACK_SEEN)
 
@@ -77,7 +77,7 @@ def _gemm_ok(*mats: Tensor) -> bool:
                 _FALLBACK_SEEN.add(key)
                 import logging
                 logging.getLogger(__name__).warning(
-                    "alpa_b200: GEMM operand %s (strides %s) is outside the sm_100a kernel's TMA constraints (%s): "
+                    "alpa_b200: GEMM operand %s (strides %s) is outside the sm_90a kernel's TMA constraints (%s): "
                     "this call uses the PyTorch library kernel", tuple(m.shape), tuple(m.stride()), bad)
             return False
     return True
@@ -791,7 +791,7 @@ def dropout_like(x: Tensor, p: float, seed: Tensor, stream: int = 0, training: b
 def linear_decode(x: Tensor, w: Tensor, w_scale: Optional[Tensor], b: Optional[Tensor] = None, act: str = "none",
                   residual: Optional[Tensor] = None, ln: Optional[Tuple[Tensor, Tensor, float]] = None) -> Tensor:
     """y = act(LN(x) @ W^T * w_scale + b) (+ residual) for a handful of tokens (decode): weight-streaming GEMV on
-    sm_100a (the streamed fp8 / bf16 weight bytes go to the tensor cores unconverted; with fp8 weights the activations
+    sm_90a (the streamed fp8 / bf16 weight bytes go to the tensor cores unconverted; with fp8 weights the activations
     are quantised per token to e4m3 inside the kernel, like the prefill fp8 GEMM; no tile padding); not
     differentiable.  x: [..., K] with at most 8 rows in total.  `ln` = (gamma, beta, eps) layer-normalises x inside the
     kernel's prologue (one launch less per projection); None = x is used as is."""
@@ -822,7 +822,7 @@ def linear_decode(x: Tensor, w: Tensor, w_scale: Optional[Tensor], b: Optional[T
 
 
 def linear_fp8(x: Tensor, w_fp8: Tensor, w_scale: Tensor, b: Optional[Tensor] = None, act: str = "none") -> Tensor:
-    """y = act(x @ (w_fp8 * w_scale[:, None])^T + b).  On sm_100a the activations are quantised per token to e4m3
+    """y = act(x @ (w_fp8 * w_scale[:, None])^T + b).  On sm_90a the activations are quantised per token to e4m3
     and the product runs on the fp8 tensor cores (`kind::f8f6f4`), scales applied in the epilogue; elsewhere the
     weights are dequantised (same maths up to the activation rounding)."""
     if x.is_cuda and global_config.use_native_kernels:
@@ -850,7 +850,7 @@ def _pack_native_ok(views: List[Tensor], flat: Tensor) -> bool:
 
 
 def pack_tiles(views: List[Tensor], flat: Optional[Tensor] = None) -> Tensor:
-    """Gather strided slices into one uint8 staging buffer (one launch on sm_100a: pack_sm100.cu)."""
+    """Gather strided slices into one uint8 staging buffer (one launch on sm_90a: pack_sm90.cu)."""
     if flat is None:
         flat = torch.empty(packed_nbytes(views), dtype=torch.uint8, device=views[0].device)
     if views and _pack_native_ok(views, flat):
@@ -878,7 +878,7 @@ def unpack_tiles(flat: Tensor, views: List[Tensor]) -> None:
 
 # =================================================================================================
 # block-scaled MXFP8 (OCP microscaling): e4m3 elements + one UE8M0 scale per 32 K elements; the scales are applied
-# inside the tensor core (tcgen05.mma kind::mxf8f6f4.block_scale, gemm_mxfp8_sm100.cu).  Scale factors are stored in
+# inside the tensor core (one wgmma per 32-element block with the scales folded in registers, gemm_sm90.cu).  Scale factors are stored in
 # the atom layout the instruction reads: [ceil(rows/128), ceil(K/128), 512] bytes, byte (r, j) of an atom at
 # (r % 32) * 16 + (r // 32) * 4 + j  (r = row inside the 128-row group, j = K block inside the 128-element slice).
 # =================================================================================================
@@ -937,8 +937,8 @@ def dequantize_mxfp8(q: Tensor, sf: Tensor) -> Tensor:
 
 
 def linear_mxfp8(x: Tensor, w_q: Tensor, w_sf: Tensor, b: Optional[Tensor] = None, act: str = "none") -> Tensor:
-    """y = act(x @ dequant(w_q, w_sf)^T + b) with block-scaled fp8 operands.  On sm_100a the activations are
-    block-quantised on the fly and the product runs on `tcgen05.mma.kind::mxf8f6f4.block_scale` (scales in tensor
+    """y = act(x @ dequant(w_q, w_sf)^T + b) with block-scaled fp8 operands.  On sm_90a the activations are
+    block-quantised on the fly and the product runs on `wgmma` e4m3 with the block scales folded in per K = 32 step (scales in
     memory); elsewhere both operands are dequantised -- the same maths, activation rounding included."""
     K, N = x.shape[-1], w_q.shape[0]
     x2 = _as2d(x)
@@ -1012,7 +1012,7 @@ def moe_top2_route(gates: Tensor, capacity: int) -> Tuple[Tensor, Tensor]:
         if ops.native_available():
             return tuple(_native().moe_top2_route(gates.float().contiguous(), C))
         if not ops.allow_fallback():
-            raise RuntimeError("alpa_b200: sm_100a extension missing for moe_top2_route")
+            raise RuntimeError("alpa_b200: sm_90a extension missing for moe_top2_route")
     idx1 = gates.argmax(-1)
     mask1 = F.one_hot(idx1, E)
     idx2 = (gates * (1 - mask1)).argmax(-1)
@@ -1325,7 +1325,7 @@ pipeline_marker.register_autograd(_marker_bwd, setup_context=_marker_setup)
 # Calling a `torch.library.custom_op` goes through the PyTorch dispatcher and the custom-op Python trampoline
 # (tens to hundreds of microseconds per call); the traced graph needs that, an executor replaying an already planned
 # program does not.  `DIRECT_IMPL` maps every alpa_b200 OpOverload to its plain Python implementation (which launches
-# the sm_100a kernel), `fast` exposes the same functions by name for inference code that never differentiates.
+# the sm_90a kernel), `fast` exposes the same functions by name for inference code that never differentiates.
 def _collect_direct():
     from torch._library.custom_ops import CustomOpDef
     table, ns = {}, {}

@@ -1,10 +1,10 @@
-"""Self-check of the newest hot-path kernel choice in a throw-away process.
+"""Self-check of the default attention forward configuration in a throw-away process.
 
     python -m alpa_b200.ops.selfcheck attention_fwd            # prints "selfcheck attention_fwd: ok | FAIL ..."
 
 `select_attention_forward()` runs it (on this rank's GPU) before a long job touches CUDA and, if the check fails, times
 out or the process dies (a device-side trap poisons the CUDA context, which is why it must not run in the caller's
-process), pins the attention forward to the previous generation via ALPA_B200_ATTN_FWD.  bench.py and
+process), pins the attention forward to its 64-query-tile configuration ("gen2") via ALPA_B200_ATTN_FWD.  bench.py and
 __graft_entry__.smoke() call it; the result is reported in bench.py's JSON (`config.attention_fwd_kernel`)."""
 import os
 import subprocess
@@ -39,7 +39,7 @@ def _check_attention_fwd() -> str:
 
 
 def select_attention_forward(timeout: float = 180.0) -> str:
-    """Returns the forward kernel generation that will be used for head dim 64 ("gen4" or "gen2")."""
+    """Returns the forward configuration that will be used: "gen4" (128-query tiles, the default) or "gen2"."""
     if os.environ.get("ALPA_B200_ATTN_FWD"):
         return os.environ["ALPA_B200_ATTN_FWD"]            # the user chose
     env = dict(os.environ)
@@ -63,7 +63,7 @@ def select_attention_forward(timeout: float = 180.0) -> str:
     if ok:
         return "gen4"
     import logging
-    logging.getLogger(__name__).warning("attention forward self-check failed (%s): using the generation-2 kernel", detail)
+    logging.getLogger(__name__).warning("attention forward self-check failed (%s): using 64-query tiles", detail)
     os.environ["ALPA_B200_ATTN_FWD"] = "gen2"
     return "gen2"
 

@@ -377,7 +377,7 @@ class PipeshardDriverExecutable:
     # ---- native communication groups (csrc/comm_group.cpp): per-pair communicators, per-direction streams, uuid events
     def _send_native(self, task, pm, shards):
         """The tiles for one peer are packed into ONE staging buffer by one kernel on the compute stream (so they are
-        ordered after the producing stage by construction; `ops.pack_tiles`, pack_sm100.cu); one uuid event marks "all
+        ordered after the producing stage by construction; `ops.pack_tiles`, pack_sm90.cu); one uuid event marks "all
         packed" and each pair group's stream waits for exactly that before its send -- one message per peer, and the
         host and the compute stream never wait (reference: alpa_nccl_wrapper.cc:140-175)."""
         from alpa_b200 import ops

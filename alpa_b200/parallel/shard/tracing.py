@@ -1,7 +1,7 @@
 """Front-end tracing: a Python train/eval step -> one flat fx graph of core-ATen + alpa_b200 primitives.
 
 Reference: alpa/util.py:868-903 (trace_jaxpr_with_micro_batch) and :335-365 (jaxpr_to_hlo).  The
-B200-native front end is torch: the step function is executed once on fake tensors under
+H100-native front end is torch: the step function is executed once on fake tensors under
 ``make_fx``; ``alpa_b200.grad`` calls ``torch.autograd.grad`` *inside* the traced function so the
 graph contains forward, backward and the optimizer update, exactly like the reference's jaxpr.
 """

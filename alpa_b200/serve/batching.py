@@ -5,7 +5,7 @@ Reference: examples/llm_serving/model/opt_model_1d.py (PromptStatus:480, Prompt:
 enter_prompts / next / update / get_results / get_latency, pad/unpad:716-738) and wrapper_1d.py (InputPoolConfig:28,
 SequenceGenerator:34 generate / generate_by_batch).  The reference's cache bookkeeping lives in an external C++
 package; here it is `alpa_b200._planner.KVCacheManager` (alpa_b200/csrc/serving_runtime.cpp) and the attention over
-the ragged batch is `ops.ragged_attention` (sm_100a kernel).
+the ragged batch is `ops.ragged_attention` (sm_90a kernel).
 """
 from __future__ import annotations
 

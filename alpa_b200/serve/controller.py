@@ -6,7 +6,7 @@ replicas; Controller:96 -- register_model:132, create_replica:149, handle_asgi:1
 forwards the request; run_controller:280 starts uvicorn), alpa/serve/http_util.py (ASGI receive/response plumbing),
 alpa/serve/run.py.
 
-B200 design: no actor framework.  A mesh group is a set of ranks of the torchrun world; the controller lives on rank
+H100 design: no actor framework.  A mesh group is a set of ranks of the torchrun world; the controller lives on rank
 0 of the node and calls replicas in-process (single-GPU models) or broadcasts the request to the ranks of the
 replica's tensor-parallel group (`SpmdReplica`), which all execute the same `handle_request`.  The HTTP side is a
 plain ASGI application (served by uvicorn when launched through `run_controller`).

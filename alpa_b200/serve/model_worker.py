@@ -4,7 +4,7 @@ Reference: examples/llm_serving/launch_model_worker.py (LangModelWorker:36 -- `c
 per-auth-group queues drained through NestedScheduler(WeightedRoundRobin) :90-112, a `batch_loop` :114 that forms
 static batches of up to `max_bs` generate requests and serves logprob requests one at a time, request logging).
 
-B200 design: the batch is not static.  The loop owns one `IterationLevelInputPool`; whenever the pool has token
+H100 design: the batch is not static.  The loop owns one `IterationLevelInputPool`; whenever the pool has token
 budget and cache room left, the scheduler's next request is admitted, and every model iteration advances all running
 sequences by one token, so short requests are not held back by long ones.  Logprob (scoring) requests run between
 iterations on the padded path.

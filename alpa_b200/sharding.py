@@ -143,7 +143,7 @@ class LogicalDeviceMesh:
 
     Mirrors the interface of the reference class (auto_sharding.py:81-169).  Cost formulas keep the
     reference's structure (so closed-form plan costs in tests carry over) but the default betas are
-    equal: through NVSwitch every peer is reachable at full NVLink-5 bandwidth.
+    equal: through NVSwitch every peer is reachable at full NVLink 4 bandwidth.
     """
 
     def __init__(self, physical_mesh, id_mesh, mesh_alpha=None, mesh_beta=None):

@@ -35,7 +35,7 @@ class InstallationTest(unittest.TestCase):
         self.assertTrue(hasattr(planner_module(), "Graph"))
         from alpa_b200 import ops
         if torch.cuda.is_available():
-            self.assertTrue(ops.native_available(), "sm_100a kernels not built: python -m alpa_b200.ops.build")
+            self.assertTrue(ops.native_available(), "sm_90a kernels not built: python -m alpa_b200.ops.build")
 
     def test_2_shard_parallel(self):
         self._run(self.alpa.ShardParallel())

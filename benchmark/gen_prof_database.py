@@ -14,7 +14,7 @@ from alpa_b200.mesh_profiling import ProfilingResultDatabase, profile_all  # noq
 
 if __name__ == "__main__":
     parser = argparse.ArgumentParser()
-    parser.add_argument("--cluster-key", type=str, default="b200-nvswitch")
+    parser.add_argument("--cluster-key", type=str, default="h100-nvswitch")
     parser.add_argument("--filename", type=str, default="prof_database.pkl")
     parser.add_argument("--max-comm-size-intra-node", type=int, default=28, help="log2 of the largest message in bytes")
     parser.add_argument("--max-comm-size-inter-node", type=int, default=26)

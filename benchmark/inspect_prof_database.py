@@ -1,7 +1,7 @@
 """Inspect (and optionally edit) a profiling database written by gen_prof_database.py
 (reference: benchmark/alpa/inspect_prof_database.py).
 
-    python benchmark/inspect_prof_database.py --filename prof_database.pkl --cluster-key b200-nvswitch --mesh 1 8
+    python benchmark/inspect_prof_database.py --filename prof_database.pkl --cluster-key h100-nvswitch --mesh 1 8
     python benchmark/inspect_prof_database.py --filename prof_database.pkl --insert-dummy 2 8      # extrapolated entry
 """
 import argparse

@@ -1,7 +1,7 @@
 """GPT training with pipeline + intra-operator parallelism (reference: examples/gpt2, benchmark_one_case_gpt_bert.py).
 
     python examples/gpt_pipeshard.py                                   # emulated 8-device cluster on CPU, tiny model
-    torchrun --nproc-per-node 8 examples/gpt_pipeshard.py --model 2.6B # 8 x B200: 2 stages x (dp2, op2)
+    torchrun --nproc-per-node 8 examples/gpt_pipeshard.py --model 2.6B # 8 x H100: 2 stages x (dp2, op2)
 """
 import argparse
 import os

@@ -2,7 +2,7 @@
 SequenceGenerator, get_model(model_name, path, batch_size, cache_size)).
 
 The engine itself is `alpa_b200.serve.batching.SequenceGenerator` (ragged 1-D token batches over a slot-addressed KV
-cache, C++ cache manager, sm_100a ragged attention kernel); this module keeps the example-level entry point and the
+cache, C++ cache manager, sm_90a ragged attention kernel); this module keeps the example-level entry point and the
 return convention of the reference: `generate(...)` -> (output ids, per-sequence latency)."""
 from __future__ import annotations
 

@@ -5,7 +5,7 @@ generated tokens/s and the mean / p90 request latency.  Static batching pads eve
 runs until its longest request finishes; the continuous engine retires requests individually.
 
     python scripts/bench_serving_continuous.py --model opt-125m --device cpu --requests 16      # smoke run on CPU
-    python scripts/bench_serving_continuous.py --model opt-2.7b --weight-dtype fp8 --requests 256 (on a B200)
+    python scripts/bench_serving_continuous.py --model opt-2.7b --weight-dtype fp8 --requests 256 (on an H100)
 """
 import argparse
 import json

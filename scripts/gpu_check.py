@@ -1,4 +1,4 @@
-"""On-GPU numerics + speed checks for the sm_100a kernel library (run under gpurun).
+"""On-GPU numerics + speed checks for the sm_90a kernel library.
 
 usage: python scripts/gpu_check.py <section> [...]   sections: gemm gemm_bench misc attn all
 Each section prints PASS/FAIL lines; exit code is non-zero on any FAIL.
@@ -319,60 +319,14 @@ def sec_moe():
     print(f"BENCH moe expert bmm [{E},{G * C},{M}]x[{E},{M},{H}]: {t * 1e3:.1f} us {2.0 * E * G * C * M * H / t / 1e9:.0f} TFLOPS")
 
 
-def sec_gemm2():
-    """CTA-pair (cta_group::2) GEMM: numerics for every operand major / epilogue, speed vs the 1-CTA kernel and cuBLAS."""
-    torch.manual_seed(11)
-    for (M, N, K) in [(256, 256, 64), (512, 512, 256), (1024, 768, 520), (384, 264, 128), (2048, 2048, 2048)]:
-        for ta in (False, True):
-            for tb in (False, True):
-                a = torch.randn((K, M) if ta else (M, K), device=dev, dtype=torch.bfloat16)
-                b = torch.randn((K, N) if tb else (N, K), device=dev, dtype=torch.bfloat16)
-                ref = (a.float().t() if ta else a.float()) @ (b.float() if tb else b.float().t())
-                try:
-                    c = _C.gemm(a, b, ta, tb, block_n=2)
-                    torch.cuda.synchronize()
-                except Exception as ex:  # noqa: BLE001
-                    print(f"FAIL gemm2 M{M} N{N} K{K} ta={int(ta)} tb={int(tb)}: {ex}")
-                    FAILS.append("gemm2-exc")
-                    return
-                check(f"gemm2 M{M} N{N} K{K} ta={int(ta)} tb={int(tb)}", c, ref, 0.05 * (K ** 0.5), 2e-2)
-    M, N, K = 1024, 1024, 512
-    a = torch.randn(M, K, device=dev, dtype=torch.bfloat16)
-    b = torch.randn(N, K, device=dev, dtype=torch.bfloat16)
-    bias = torch.randn(N, device=dev, dtype=torch.bfloat16)
-    res = torch.randn(M, N, device=dev, dtype=torch.bfloat16)
-    aux = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-    c = _C.gemm(a, b, False, False, bias=bias, residual=res, aux_out=aux, act=1, block_n=2)
-    z = a.float() @ b.float().t() + bias.float()
-    check("gemm2 bias+gelu+residual", c, torch.nn.functional.gelu(z) + res.float(), 0.6, 2e-2)
-    check("gemm2 aux_out", aux, z, 0.6, 2e-2)
-    acc = torch.randn(M, N, device=dev, dtype=torch.float32)
-    acc0 = acc.clone()
-    _C.gemm(a, b, False, False, out=acc, accumulate=True, block_n=2)
-    check("gemm2 fp32 accumulate", acc, acc0 + a.float() @ b.float().t(), 0.6, 2e-2)
-    flush = torch.empty(256 * 1024 * 1024, device=dev, dtype=torch.uint8)
-    for (name, M, N, K, ta, tb) in [("8192^3", 8192, 8192, 8192, False, False), ("fc1 fwd", 16384, 8192, 2048, False, False),
-                                    ("fc1 dgrad", 16384, 2048, 8192, False, True), ("fc1 wgrad", 8192, 2048, 16384, True, True),
-                                    ("qkv fwd", 16384, 6144, 2048, False, False), ("proj fwd", 16384, 2048, 2048, False, False)]:
-        a = torch.randn((K, M) if ta else (M, K), device=dev, dtype=torch.bfloat16)
-        b = torch.randn((K, N) if tb else (N, K), device=dev, dtype=torch.bfloat16)
-        t2 = timeit(lambda: _C.gemm(a, b, ta, tb, block_n=2), flush=flush)
-        t1 = timeit(lambda: _C.gemm(a, b, ta, tb, block_n=256), flush=flush)
-        am = a.t() if ta else a
-        bm = b if tb else b.t()
-        tc = timeit(lambda: torch.matmul(am, bm), flush=flush)
-        fl = 2.0 * M * N * K
-        print(f"BENCH gemm {name}: 2-CTA {t2 * 1e3:.1f} us {fl / t2 / 1e9:.0f} TFLOPS | 1-CTA {t1 * 1e3:.1f} us "
-              f"{fl / t1 / 1e9:.0f} TFLOPS | cuBLAS {tc * 1e3:.1f} us {fl / tc / 1e9:.0f} TFLOPS", flush=True)
-
-
 def _bench_note(line):
-    """Timing lines of the GPU checks, kept in a file (pytest / tail filters drop stdout)."""
+    """Timing lines of the GPU checks; also appended to $ALPA_B200_BENCH_NOTES when set (pytest drops stdout)."""
     import os
     print("BENCH " + line, flush=True)
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open("gpurun_out/gpu_check_bench.txt", "a") as f:
-        f.write(line + "\n")
+    path = os.environ.get("ALPA_B200_BENCH_NOTES")
+    if path:
+        with open(path, "a") as f:
+            f.write(line + "\n")
 
 
 def sec_gemv():
@@ -570,8 +524,6 @@ if __name__ == "__main__":
             sec_moe()
         if s in ("fp8",):
             sec_fp8()
-        if s in ("gemm2",):
-            sec_gemm2()
         if s in ("ragged",):
             sec_ragged()
     print(f"done in {time.time() - t0:.1f}s; FAILS={FAILS}")

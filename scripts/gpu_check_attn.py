@@ -27,7 +27,7 @@ def run(check, timeit, FAILS, bwd=True):
     cases = [(2, 4, 128, 128, 64, False), (2, 4, 256, 256, 64, False), (1, 3, 384, 384, 64, True),
              (2, 2, 200, 200, 64, False), (1, 2, 328, 328, 64, True), (2, 2, 256, 256, 128, False),
              (1, 2, 512, 512, 128, True), (1, 2, 256, 256, 80, False), (1, 4, 1024, 1024, 64, False),
-             (1, 2, 128, 512, 64, False)]
+             (1, 2, 128, 512, 64, False), (2, 2, 100, 300, 64, True), (1, 2, 64, 200, 128, True)]
     for (B, H, Sq, Sk, D, causal) in cases:
         qkv = torch.randn(B, max(Sq, Sk), 3, H, D, device=dev, dtype=torch.bfloat16)
         q, k, v = qkv[:, :Sq, 0], qkv[:, :Sk, 1], qkv[:, :Sk, 2]
@@ -58,6 +58,29 @@ def run(check, timeit, FAILS, bwd=True):
             check(f"attn bwd dq {tag}", dq, qf.grad, 5e-2, 3e-2)
             check(f"attn bwd dk {tag}", dk, kf.grad, 5e-2, 3e-2)
             check(f"attn bwd dv {tag}", dv, vf.grad, 5e-2, 3e-2)
+    # device-side KV length (prefill into a cache): only the first kv_len keys are visible, the causal shift uses kv_len
+    for (B, H, Sq, Smax, kvl, D, causal) in [(2, 2, 40, 256, 170, 64, True), (1, 3, 64, 192, 100, 128, False)]:
+        q = torch.randn(B, Sq, H, D, device=dev, dtype=torch.bfloat16)
+        k = torch.randn(B, Smax, H, D, device=dev, dtype=torch.bfloat16)
+        v = torch.randn(B, Smax, H, D, device=dev, dtype=torch.bfloat16)
+        scale = 1.0 / math.sqrt(D)
+        o, lse = _C.attention_fwd(q, k, v, scale, causal, torch.tensor([kvl], device=dev, dtype=torch.int32))
+        o_ref, lse_ref = ref_attn(q, k[:, :kvl], v[:, :kvl], scale, causal)
+        tag = f"kv_len B{B} H{H} Sq{Sq} Smax{Smax} kv_len{kvl} D{D} causal={int(causal)}"
+        check(f"attn fwd o {tag}", o, o_ref, 2e-2, 2e-2)
+        check(f"attn fwd lse {tag}", lse, lse_ref, 2e-2, 1e-3)
+    # the 64-query-tile configuration the self-check falls back to (selected per process by ALPA_B200_ATTN_FWD)
+    import os
+    import subprocess
+    import sys
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    env = dict(os.environ, ALPA_B200_ATTN_FWD="gen2", PYTHONPATH=root + os.pathsep + os.environ.get("PYTHONPATH", ""))
+    r = subprocess.run([sys.executable, "-m", "alpa_b200.ops.selfcheck", "attention_fwd"], env=env, cwd=root,
+                       capture_output=True, text=True, timeout=300)
+    line = (r.stdout.strip().splitlines() or ["no output"])[-1]
+    print(f"attn fwd 64-query tiles: {line}")
+    if r.returncode != 0 or " ok" not in line:
+        FAILS.append("attn-gen2")
     # speed (GPT-1.3B: 32 heads x 64; 15B: 40 heads x 128)
     flush = torch.empty(256 * 1024 * 1024, device=dev, dtype=torch.uint8)
     for (B, H, S, D, causal) in [(8, 32, 1024, 64, False), (8, 32, 1024, 64, True), (8, 40, 1024, 128, False),
@@ -80,37 +103,3 @@ def run(check, timeit, FAILS, bwd=True):
             do = torch.randn_like(o)
             t = timeit(lambda: _C.attention_bwd(do, q, k, v, o, lse, scale, causal), flush=flush)
             print(f"BENCH attn bwd B{B} H{H} S{S} D{D} causal={int(causal)}: {t:.3f} ms {2.5 * fl / t / 1e9:.1f} TFLOPS", flush=True)
-
-
-def trace_fwd(B=8, H=32, S=1024, D=64):
-    """Timeline of one CTA of the third-generation forward (ALPA_B200_ATTN_FWD=gen3): clock64 stamps relative to the
-    first event, per key tile."""
-    qkv = torch.randn(B, S, 3, H, D, device=dev, dtype=torch.bfloat16)
-    q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
-    for _ in range(3):
-        _C.attention_fwd(q, k, v, D ** -0.5, False)
-    tr = torch.zeros(1024, dtype=torch.int64, device=dev)
-    _C.attention_fwd(q, k, v, D ** -0.5, False, None, tr)
-    torch.cuda.synchronize()
-    t = tr.cpu().view(-1, 8)
-    nz = t[t > 0]
-    if nz.numel() == 0:
-        print("TRACE: no events (kernel is not the gen3 forward?)")
-        return
-    t0 = int(nz.min())
-    ntiles = (S + 127) // 128
-    print("TRACE softmax: tile set | S landed | loaded+max | token | exp done | P signalled   (clk since first event)")
-    for j in range(ntiles):
-        s_, n = j & 1, j >> 1
-        r = t[s_ * 32 + n]
-        print(f"TRACE   tile {j} set {s_}: " + " ".join(f"{int(x) - t0:7d}" if x > 0 else "      -" for x in r[:5]))
-    print("TRACE mma: tile | P ready | PV issued | S buffer free | S(j+2) issued")
-    for j in range(ntiles):
-        r = t[64 + j]
-        print(f"TRACE   tile {j}: " + " ".join(f"{int(x) - t0:7d}" if x > 0 else "      -" for x in r[:4]))
-
-
-if __name__ == "__main__":
-    import sys
-    if len(sys.argv) > 1 and sys.argv[1] == "trace":
-        trace_fwd()

@@ -1,5 +1,5 @@
-"""First hardware check of the block-scaled MXFP8 path (gemm_mxfp8_sm100.cu): the on-the-fly quantiser against the
-PyTorch reference (bit exact), the tcgen05 `kind::mxf8f6f4.block_scale` GEMM against an fp32 matmul of the dequantised
+"""First hardware check of the block-scaled MXFP8 path (gemm_sm90.cu): the on-the-fly quantiser against the
+PyTorch reference (bit exact), the block-scaled MXFP8 `wgmma` GEMM against an fp32 matmul of the dequantised
 operands, and device-timed throughput next to the per-token x per-channel fp8 GEMM.  Written after the round's GPU
 budget was spent: run it in a throw-away process with a timeout (tests/test_zzz_gpu_first_hardware_runs.py does).
     python scripts/gpu_check_mxfp8.py"""

@@ -1,4 +1,4 @@
-"""First hardware run of the resharding pack / unpack kernel (pack_sm100.cu) against the PyTorch reference, plus the
+"""First hardware run of the resharding pack / unpack kernel (pack_sm90.cu) against the PyTorch reference, plus the
 device-timed cost of one packed launch next to one `.contiguous()` copy per tile.
     python scripts/gpu_check_pack.py"""
 import os

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA GPU (B200); run with -m gpu")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA GPU (H100); run with -m gpu")
 
 
 def pytest_collection_modifyitems(config, items):

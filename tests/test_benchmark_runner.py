@@ -38,14 +38,13 @@ def test_benchmark_one_case_modes(mode, args, nmb, ngpu):
         alpa.shutdown()
 
 
-def test_resharding_benchmark_plans_show_load_balance_and_allgather_effects():
+def test_resharding_benchmark_plans_show_load_balance_and_allgather_effects(tmp_path):
     """benchmark/resharding (plan-only): load balancing halves the busiest sender for a replicated source, the local
     all-gather halves the cross-mesh bytes for a replicated destination (reference: benchmark/alpa/resharding)."""
     import subprocess
     import sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    out = str(os.path.join(root, "gpurun_out", "_resharding_plan_test.jsonl"))
-    os.makedirs(os.path.dirname(out), exist_ok=True)
+    out = str(tmp_path / "resharding_plan.jsonl")
     r = subprocess.run([sys.executable, "benchmark/resharding/benchmark_cross_mesh_resharding.py", "--suite", "n-to-m",
                         "--plan-only", "--json", out], cwd=root, capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stderr[-2000:]

@@ -39,8 +39,7 @@ def test_documented_repo_paths_exist():
             if any(ch in ref for ch in "{}*"):
                 continue
             cand = os.path.join(ROOT, ref)
-            in_reference = os.path.exists(os.path.join("/root/reference", ref)) or \
-                ref.startswith(("benchmark/alpa/", "examples/llm_serving/benchmark/", "docs/gallery/"))
+            in_reference = ref.startswith(("benchmark/alpa/", "examples/llm_serving/benchmark/", "docs/gallery/"))
             if not (os.path.exists(cand) or glob.glob(cand + "*") or in_reference):
                 missing.append((os.path.relpath(path, ROOT), ref))
     assert not missing, missing

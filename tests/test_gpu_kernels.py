@@ -1,4 +1,4 @@
-"""Numerics of the sm_100a kernels against fp32 PyTorch references (run with -m gpu on a B200)."""
+"""Numerics of the sm_90a kernels against fp32 PyTorch references (run with -m gpu on an H100)."""
 import importlib
 
 import pytest
@@ -16,7 +16,7 @@ def _run(section):
 
 def test_native_extension_loaded():
     from alpa_b200 import ops
-    assert ops.native_available(), "sm_100a extension must be built in-tree (python -m alpa_b200.ops.build)"
+    assert ops.native_available(), "sm_90a extension must be built in-tree (python -m alpa_b200.ops.build)"
     assert hasattr(ops.native_module(), "gemm")
 
 

@@ -1,5 +1,5 @@
-"""Block-scaled MXFP8 (OCP microscaling) maths shared by the sm_100a kernel and its CPU reference: exponent choice,
-the scale-factor atom layout `tcgen05.cp` / `tcgen05.mma.block_scale` read, and the reference linear."""
+"""Block-scaled MXFP8 (OCP microscaling) maths shared by the sm_90a kernel and its CPU reference: exponent choice,
+the scale-factor atom layout the MXFP8 GEMM reads, and the reference linear."""
 import torch
 
 from alpa_b200 import ops

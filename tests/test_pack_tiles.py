@@ -1,5 +1,5 @@
 """`ops.pack_tiles` / `ops.unpack_tiles`: the tiles of a resharding task for one peer as one 16-byte-aligned staging
-buffer (reference of pack_sm100.cu; the kernel itself is checked by scripts/gpu_check_pack.py)."""
+buffer (reference of pack_sm90.cu; the kernel itself is checked by scripts/gpu_check_pack.py)."""
 import torch
 
 from alpa_b200 import ops

@@ -131,16 +131,16 @@ def test_profiling_database_estimate(tmp_path):
         table[(4, "bf16")] = [(float(n), 1e-6 + n / 400e9) for n in sizes]
     prof.dot_cost_dict[("bf16",)] = [(2.0 * n ** 3, 2.0 * n ** 3 / 1.2e15) for n in (1024, 4096)]
     db = ProfilingResultDatabase()
-    db.update_one_mesh("b200", (1, 4), prof)
+    db.update_one_mesh("h100", (1, 4), prof)
     path = str(tmp_path / "prof.pkl")
     db.save(path)
     db2 = ProfilingResultDatabase()
     db2.load(path)
-    c_small = estimate_stage_cost_from_db(db2, "b200", (1, 4), 1e12, [("all_reduce", 4, float(1 << 20))])
-    c_big = estimate_stage_cost_from_db(db2, "b200", (1, 4), 4e12, [("all_reduce", 4, float(1 << 24))])
+    c_small = estimate_stage_cost_from_db(db2, "h100", (1, 4), 1e12, [("all_reduce", 4, float(1 << 20))])
+    c_big = estimate_stage_cost_from_db(db2, "h100", (1, 4), 4e12, [("all_reduce", 4, float(1 << 24))])
     assert 0 < c_small < c_big
     # interpolation inside the table, linear extrapolation above it; unknown mesh -> analytic model
-    r = db2.query("b200", (1, 4))
+    r = db2.query("h100", (1, 4))
     mid = r.estimate_all_reduce(4, "bf16", 3 * (1 << 19))
     assert r.estimate_all_reduce(4, "bf16", 1 << 20) < mid * 1.0001 or mid > 0
     assert abs(r.estimate_all_reduce(4, "bf16", 1 << 25) - 2 * r.estimate_all_reduce(4, "bf16", 1 << 24)) < 1e-9

@@ -1,6 +1,6 @@
 """First hardware runs of code written after this round's GPU budget was spent (runs last).  Each check runs in a
 throw-away process with a timeout, so a wrong barrier protocol cannot hang the session, and is marked
-xfail(strict=False): the suite reports XPASS when the new path works on the B200 and XFAIL -- not a red suite -- when
+xfail(strict=False): the suite reports XPASS when the new path works on the H100 and XFAIL -- not a red suite -- when
 it does not; nothing on a default execution path depends on these kernels (both are opt-in)."""
 import os
 import subprocess
@@ -46,7 +46,7 @@ def _run_inner(script, timeout, *args):
     return r
 
 
-@pytest.mark.xfail(strict=False, reason="block-scaled MXFP8 GEMM (tcgen05.mma kind::mxf8f6f4.block_scale): first hardware run")
+@pytest.mark.xfail(strict=False, reason="block-scaled MXFP8 GEMM (wgmma, scales folded per K block): first hardware run")
 def test_mxfp8_block_scaled_gemm_first_hardware_run():
     r = _run("gpu_check_mxfp8.py", 150)
     assert r.returncode == 0 and "mxfp8 check: ok" in r.stdout
@@ -76,7 +76,7 @@ def test_grad_accumulation_and_remat_first_hardware_run():
     assert r.returncode == 0 and "train feature check: ok" in r.stdout
 
 
-@pytest.mark.xfail(strict=False, reason="resharding pack / unpack kernel (pack_sm100.cu): first hardware run")
+@pytest.mark.xfail(strict=False, reason="resharding pack / unpack kernel (pack_sm90.cu): first hardware run")
 def test_resharding_pack_kernel_first_hardware_run():
     r = _run("gpu_check_pack.py", 120)
     assert r.returncode == 0 and "pack check: ok" in r.stdout
@@ -85,7 +85,7 @@ def test_resharding_pack_kernel_first_hardware_run():
 @pytest.mark.xfail(strict=False, reason="informational: GEMM / attention timings of the kernels at HEAD on this box")
 def test_kernel_timings_at_head():
     """Not a validation (the numerics of these kernels are checked by tests/test_gpu_kernels.py): re-runs the timing
-    sections of the GPU check scripts so that the session log carries TFLOPS of the tcgen05 GEMM (1-CTA / CTA pair /
-    cuBLAS) and of the attention forward / backward as built from this commit."""
-    r = _run("gpu_check.py", 240, "gemm2", "attn")
+    sections of the GPU check scripts so that the session log carries TFLOPS of the wgmma GEMM (against cuBLAS) and of
+    the attention forward / backward as built from this commit."""
+    r = _run("gpu_check.py", 240, "gemm_bench", "attn")
     assert r.returncode == 0
