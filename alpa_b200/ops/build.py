@@ -49,11 +49,22 @@ def _hash(paths, extra="") -> str:
     return h.hexdigest()[:16]
 
 
-def _run(cmd, what):
+# ptxas "wgmma pipeline crossing function boundary": a call anywhere in a kernel (printf included) makes ptxas wait
+# for every wgmma.mma_async of that kernel to finish before the next one issues.  The build refuses it.
+SERIALIZED_WGMMA = "C7510"
+
+
+def _run(cmd, what, out=None):
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         sys.stderr.write(f"[alpa_b200.build] {what} failed:\n{' '.join(map(str, cmd))}\n{r.stdout}\n{r.stderr}\n")
         raise RuntimeError(f"{what} failed")
+    if SERIALIZED_WGMMA in r.stdout + r.stderr:
+        if out is not None:
+            Path(out).unlink(missing_ok=True)  # not cached: the next build reports it again
+        sys.stderr.write(f"[alpa_b200.build] {what}: serialized wgmma ({SERIALIZED_WGMMA}):\n"
+                         f"{' '.join(map(str, cmd))}\n{r.stdout}\n{r.stderr}\n")
+        raise RuntimeError(f"{what}: ptxas serialized wgmma ({SERIALIZED_WGMMA}); remove the call from the kernel")
     return r
 
 
@@ -74,7 +85,7 @@ def _compile_objects(jobs):
     if not todo:
         return
     with cf.ThreadPoolExecutor(max_workers=min(8, len(todo))) as ex:
-        futs = [ex.submit(_run, cmd, what) for cmd, _, what in todo]
+        futs = [ex.submit(_run, cmd, what, out) for cmd, out, what in todo]
         for f in futs:
             f.result()
 

@@ -13,6 +13,8 @@
 //
 // Replaces: NCCL thunks after cuBLAS GEMMs in the reference (K3/K5/K10 of SURVEY.md §2.5,
 // XLA/service/gpu/nccl_all_reduce_thunk.cc:103-121, :434-458, nccl_all_gather_thunk.cc:73-91).
+#include <stdio.h>
+
 #include "kernels.h"
 #include "pdl.h"
 #include "ptx.cuh"

@@ -25,7 +25,6 @@
 #include <stdint.h>
 
 #include <mutex>
-#include <stdio.h>
 
 #include "gemm_sm90.h"
 #include "kernels.h"
@@ -38,6 +37,7 @@ namespace ab {
 constexpr int BLOCK_M = 128;
 constexpr int kRowBytes = 128;  // K bytes per stage: 64 bf16 or 128 e4m3
 constexpr int kNumThreads = 384;
+constexpr int kGroupM = 16;  // M-blocks per band of the tile order (see tile_coords)
 
 enum : uint32_t { kMajorK = 0, kMajorMN = 1 };  // operand major (wgmma transpose flag)
 enum : int { kModeBf16 = 0, kModeFp8 = 1, kModeMx = 2 };
@@ -123,13 +123,19 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   }
   __syncthreads();
 
-  // Tile order: consecutive tile ids walk M first so concurrently resident CTAs share B panels
-  // and the whole of A stays in the 50 MB L2.
+  // Tile order: batch outermost, then bands of kGroupM M-blocks; inside a band consecutive tile ids walk M first, then
+  // N.  The CTAs resident at one time (one tile id each) then cover about kGroupM A row-panels and
+  // #SMs / kGroupM B column-panels, so both operands are fetched from DRAM about once per wave and reused from L2.
+  // Walking M over the whole matrix instead would re-read all of A every wave once A outgrows the 50 MB L2, which it
+  // does at training shapes (16384 tokens x K = 2048 bf16 is already 64 MB).  The last band holds the M tail.
   auto tile_coords = [&](int tile, int& b, int& m_blk, int& n_blk) {
     b = tile / tiles_per_batch;
     const int t = tile - b * tiles_per_batch;
-    n_blk = t / num_m_blocks;
-    m_blk = t - n_blk * num_m_blocks;
+    const int first = t / (kGroupM * num_n_blocks) * kGroupM;
+    const int rows = min(kGroupM, num_m_blocks - first);
+    const int r = t - first * num_n_blocks;
+    n_blk = r / rows;
+    m_blk = first + (r - n_blk * rows);
     if (ep.m_block_rotate) m_blk = (m_blk + ep.m_block_rotate) % num_m_blocks;
   };
 
@@ -143,14 +149,11 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         tile_coords(tile, b, m_blk, n_blk);
         const int m0 = m_blk * BLOCK_M, n0 = n_blk * BLOCK_N;
         if (ep.a_ready != nullptr && (m_blk < ep.a_own_lo || m_blk >= ep.a_own_hi)) {
-          // all-gather -> GEMM: wait for the peer that owns these rows to publish them
+          // all-gather -> GEMM: wait for the peer that owns these rows to publish them (silent trap: see mbar_wait)
           uint32_t spins = 0;
           while (ld_acquire_sys(ep.a_ready + m_blk) < ep.a_ready_epoch) {
             __nanosleep(64);
-            if (++spins > (1u << 24)) {
-              printf("alpa_b200: a_ready watchdog m_blk %d\n", m_blk);
-              __trap();
-            }
+            if (++spins > (1u << 24)) __trap();
           }
           asm volatile("fence.proxy.async;\n" ::: "memory");
         }

@@ -8,7 +8,6 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdio.h>
 
 namespace ab {
 
@@ -60,7 +59,9 @@ __device__ __forceinline__ uint32_t mbar_try_wait(uint64_t* bar, uint32_t parity
       : "memory");
   return ok;
 }
-// Spin with a watchdog: a protocol bug traps instead of hanging the GPU (a hung box is a strike).
+// Spin with a watchdog: a protocol bug traps instead of hanging the GPU.  The watchdog must not call a function
+// (printf included): wgmma kernels wait here, and ptxas serialises every wgmma.mma_async of a kernel that contains a
+// call (warning C7510), so the trap is silent and surfaces as a launch failure on the host.
 #ifndef AB_MBAR_WATCHDOG
 #define AB_MBAR_WATCHDOG 1
 #endif
@@ -74,10 +75,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if ((++spins & 1023u) == 0) {   // wall-clock watchdog: 10 s without progress is a protocol bug, not a wait
       unsigned long long t1;
       asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-      if (t1 - t0 > 10000000000ull) {
-        printf("alpa_b200: mbarrier watchdog block(%d,%d) thread %d\n", blockIdx.x, blockIdx.y, threadIdx.x);
-        __trap();
-      }
+      if (t1 - t0 > 10000000000ull) __trap();
     }
   }
 #else

@@ -117,31 +117,50 @@ def sec_gemm():
 
 
 def sec_gemm_bench():
+    """The 15 GEMMs of one GPT-1.3B training step on one GPU (16 x 1024 tokens, H = 2048, 4H = 8192, V = 51200), with
+    the operand majors, tile width and epilogues the step runs them with: the forward linears add the bias, fc1 also
+    applies GELU and saves the pre-activation (aux_out), and the fc2 dgrad applies dGELU from it (aux_in).  The
+    residual epilogue is not on this list: on one GPU the step adds the residual gradient in a separate kernel
+    (ALPA_B200_FUSE_DGRAD_ADD is off by default).  M = 16384 makes A larger than the 50 MB L2, as in the step.
+    cuBLAS runs the same product without the epilogue."""
     flush = torch.empty(256 * 1024 * 1024, device=dev, dtype=torch.uint8)
-    shapes = [
-        ("8192^3", 8192, 8192, 8192, False, False),
-        ("qkv 1.3B fwd", 8192, 6144, 2048, False, False),
-        ("fc1 1.3B fwd", 8192, 8192, 2048, False, False),
-        ("fc2 1.3B fwd", 8192, 2048, 8192, False, False),
-        ("proj 1.3B fwd", 8192, 2048, 2048, False, False),
-        ("fc1 dgrad (NN)", 8192, 2048, 8192, False, True),
-        ("fc1 wgrad (TN)", 8192, 2048, 8192, True, True),
-        ("lm head", 8192, 51200, 2048, False, False),
-        ("16384x8192x2048", 16384, 8192, 2048, False, False),
-    ]
-    for name, M, N, K, ta, tb in shapes:
+    T, H, I, V = 16384, 2048, 8192, 51200
+    NONE, BIAS, GELU, DGELU = "", "bias", "bias+gelu+aux_out", "dgelu"
+    shapes = []  # (name, M, N, K, trans_a, trans_b, epilogue)
+    for name, n_in, n_out in (("qkv", H, 3 * H), ("proj", H, H), ("fc1", H, I), ("fc2", I, H), ("lm head", H, V)):
+        shapes.append((f"{name} fwd", T, n_out, n_in, False, False, GELU if name == "fc1" else BIAS))
+        shapes.append((f"{name} dgrad", T, n_in, n_out, False, True, DGELU if name == "fc2" else NONE))
+        shapes.append((f"{name} wgrad", n_out, n_in, T, True, True, NONE))
+    for name, M, N, K, ta, tb, epi in shapes:
         a = torch.randn((K, M) if ta else (M, K), device=dev, dtype=torch.bfloat16)
-        b = torch.randn((K, N) if tb else (N, K), device=dev, dtype=torch.bfloat16)
+        b = torch.randn((K, N) if tb else (N, K), device=dev, dtype=torch.bfloat16) * K ** -0.5
         out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
+        kw = {}
+        if epi in (BIAS, GELU):
+            kw["bias"] = torch.randn(N, device=dev, dtype=torch.bfloat16)
+        if epi == GELU:
+            kw.update(aux_out=torch.empty(M, N, device=dev, dtype=torch.bfloat16), act=1)
+        if epi == DGELU:
+            kw.update(aux_in=torch.randn(M, N, device=dev, dtype=torch.bfloat16), act=3)
         A = a.t() if ta else a
         B = b if tb else b.t()
         ref_out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-        for bn in (256, 128):
-            t = timeit(lambda: _C.gemm(a, b, ta, tb, out=out, block_n=bn), flush=flush)
-            print(f"BENCH gemm {name} bn={bn}: {t:.3f} ms  {2 * M * N * K / t / 1e9:.1f} TFLOPS", flush=True)
+        t = timeit(lambda: _C.gemm(a, b, ta, tb, out=out, **kw), flush=flush)
         t2 = timeit(lambda: torch.matmul(A, B, out=ref_out), flush=flush)
-        print(f"BENCH cublas {name}: {t2:.3f} ms  {2 * M * N * K / t2 / 1e9:.1f} TFLOPS", flush=True)
-        check(f"bench-correct {name}", out, ref_out, 0.5, 3e-2)
+        fl = 2 * M * N * K / 1e9
+        print(f"BENCH gemm {name:12s} M={M:5d} N={N:5d} K={K:5d} {epi or '-':17s}: {t:.3f} ms {fl / t:6.1f} TFLOPS | "
+              f"cublas {t2:.3f} ms {fl / t2:6.1f} TFLOPS", flush=True)
+        ref = ref_out.float()
+        if "bias" in kw:
+            ref = ref + kw["bias"].float()
+        if epi == GELU:
+            ref = torch.nn.functional.gelu(ref)
+        if epi == DGELU:
+            z = kw["aux_in"].float().requires_grad_(True)
+            torch.nn.functional.gelu(z).backward(torch.ones_like(z))
+            ref = ref * z.grad
+        check(f"bench-correct {name}", out, ref, 0.05, 3e-2)
+        del a, b, out, ref_out, ref, kw
 
 
 def sec_misc():
