@@ -413,9 +413,15 @@ def _attn_ref(q, k, v, scale, causal):
         mask = torch.ones(Sq, Sk, device=s.device, dtype=torch.bool).tril(Sk - Sq)
         s = s.masked_fill(~mask, float("-inf"))
     lse = torch.logsumexp(s, dim=-1)
-    p = torch.exp(s - lse[..., None])
+    p = torch.exp(s - _finite_lse(lse)[..., None])
     o = torch.matmul(p, vf).permute(0, 2, 1, 3)
     return o.to(q.dtype).contiguous(), lse
+
+
+def _finite_lse(lse):
+    """lse with the -inf of rows that see no key replaced by 0: exp(s - lse) is then exp(-inf) = 0 on those rows, so
+    they get O = 0 and zero gradients (as the native kernels give) instead of exp(-inf + inf) = NaN."""
+    return lse.masked_fill(lse == float("-inf"), 0.0)
 
 
 @torch.library.custom_op("alpa_b200::attention", mutates_args=())
@@ -447,7 +453,7 @@ def attention_bwd(do: Tensor, q: Tensor, k: Tensor, v: Tensor, o: Tensor, lse: T
         Sq, Sk = s.shape[-2:]
         mask = torch.ones(Sq, Sk, device=s.device, dtype=torch.bool).tril(Sk - Sq)
         s = s.masked_fill(~mask, float("-inf"))
-    p = torch.exp(s - lse[..., None])
+    p = torch.exp(s - _finite_lse(lse)[..., None])
     dv = torch.matmul(p.transpose(-1, -2), dof)
     dp = torch.matmul(dof, vf.transpose(-1, -2))
     delta = (dof * of).sum(-1, keepdim=True)
