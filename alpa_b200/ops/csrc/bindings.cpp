@@ -76,6 +76,15 @@ Tensor gemm(const Tensor& a, const Tensor& b, bool trans_a, bool trans_b, const 
     TORCH_CHECK(!accumulate, "gemm: accumulate needs an explicit out");
   }
   TORCH_CHECK(out.size(out.dim() - 2) == g.M && out.size(out.dim() - 1) == g.N, "gemm: out shape");
+  TORCH_CHECK(out.dim() == nd && (nd == 2 || out.size(0) == g.batch), "gemm: out batch");
+  // the epilogue stores two adjacent columns at once: 4 bytes (bf16) or 8 bytes (fp32)
+  const size_t out_align = out_fp32 ? 8 : 4;
+  auto pair_aligned = [&](const Tensor& t, size_t align) {
+    return reinterpret_cast<uintptr_t>(t.data_ptr()) % align == 0 && t.stride(t.dim() - 2) % 2 == 0 &&
+           (t.dim() == 2 || t.stride(0) % 2 == 0);
+  };
+  TORCH_CHECK(pair_aligned(out, out_align), "gemm: out needs even row / batch strides and a ", out_align,
+              "-byte aligned base");
   g.ep.out = out.data_ptr();
   g.ep.ldc = out.stride(out.dim() - 2);
   g.ep.batch_stride_c = out.dim() == 3 ? out.stride(0) : 0;
@@ -83,13 +92,19 @@ Tensor gemm(const Tensor& a, const Tensor& b, bool trans_a, bool trans_b, const 
   g.ep.accumulate = accumulate ? 1 : 0;
   g.ep.alpha = (float)alpha;
   g.ep.act = (int)act;
+  if (bias.has_value() && bias->defined())
+    TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->is_contiguous() && bias->numel() == g.N &&
+                    reinterpret_cast<uintptr_t>(bias->data_ptr()) % 4 == 0,
+                "gemm: bias must be a contiguous, 4-byte aligned bf16 [N]");
   g.ep.bias = bf16_ptr(bias);
   auto same_layout = [&](const OptTensor& t, const char* name) {
     if (t.has_value() && t->defined()) {
-      TORCH_CHECK(t->dim() == out.dim() && t->stride(t->dim() - 1) == 1 &&
+      TORCH_CHECK(t->dim() == out.dim() && t->sizes() == out.sizes() && t->stride(t->dim() - 1) == 1 &&
                       t->stride(t->dim() - 2) == g.ep.ldc &&
                       (t->dim() == 2 || t->stride(0) == g.ep.batch_stride_c),
-                  "gemm: ", name, " must share the output layout");
+                  "gemm: ", name, " must share the output's sizes and layout");
+      TORCH_CHECK(t->scalar_type() == at::kBFloat16 && pair_aligned(*t, 4), "gemm: ", name,
+                  " must be bf16 with a 4-byte aligned base");
     }
   };
   same_layout(residual, "residual");
@@ -684,24 +699,60 @@ Tensor moe_combine_wgrad(const Tensor& dout, const Tensor& eo, const Tensor& exp
 }
 
 // ---- fp8 serving GEMM ---------------------------------------------------------------------------
-// y = act((quantize_rows(x) . w_fp8^T) * sx * sw + bias): x bf16 [M, K], w e4m3 [N, K], w_scale fp32 [N]
-Tensor gemm_fp8(const Tensor& x, const Tensor& w, const Tensor& w_scale, const OptTensor& bias, int64_t act) {
-  TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.stride(1) == 1, "gemm_fp8: x");
-  TORCH_CHECK(w.scalar_type() == at::kFloat8_e4m3fn && w.dim() == 2 && w.is_contiguous(), "gemm_fp8: w must be e4m3");
-  TORCH_CHECK(w_scale.scalar_type() == at::kFloat && w_scale.is_contiguous() && w_scale.numel() == w.size(0));
+// The row quantisers read x 16 bytes at a time (ld_nc_v4): every row must start on a 16-byte boundary.
+void check_rows_16b(const Tensor& x, const char* what) {
+  TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.stride(1) == 1, what,
+              ": x must be a 2-D CUDA bf16 tensor with a contiguous inner dim");
+  TORCH_CHECK(x.stride(0) % 8 == 0 && reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0, what,
+              ": x needs a row stride that is a multiple of 8 and a 16-byte aligned base");
+}
+
+// Per-row e4m3 quantisation of the activations: x bf16 [M, K] -> (q e4m3 [M, K], sx fp32 [M]), x ~ q * sx[m]
+std::vector<Tensor> quantize_e4m3(const Tensor& x) {
+  check_rows_16b(x, "quantize_e4m3");
   c10::cuda::CUDAGuard guard(x.device());
-  const int M = (int)x.size(0), K = (int)x.size(1), N = (int)w.size(0);
-  TORCH_CHECK(w.size(1) == K && K % 16 == 0 && N % 8 == 0, "gemm_fp8: shapes");
-  Tensor xq = torch::empty({M, K}, x.options().dtype(at::kByte));
+  const int M = (int)x.size(0), K = (int)x.size(1);
+  TORCH_CHECK(K % 16 == 0, "quantize_e4m3: K must be a multiple of 16");
+  Tensor q = torch::empty({M, K}, x.options().dtype(at::kFloat8_e4m3fn));
   Tensor sx = torch::empty({M}, x.options().dtype(at::kFloat));
-  AB_CHECK_RC(ab_quantize_rows_e4m3(bf16_ptr(x), xq.data_ptr<uint8_t>(), sx.data_ptr<float>(), M, K, x.stride(0),
-                                    cur_stream()), "ab_quantize_rows_e4m3");
-  Tensor out = torch::empty({M, N}, x.options());
-  AB_CHECK_RC(ab_gemm_fp8(xq.data_ptr<uint8_t>(), reinterpret_cast<const uint8_t*>(w.data_ptr()), sx.data_ptr<float>(),
-                          w_scale.data_ptr<float>(), bf16_ptr(bias), reinterpret_cast<__nv_bfloat16*>(out.data_ptr()), M,
-                          N, K, N, (int)act, cur_stream()), "ab_gemm_fp8");
-  g_launches += 2;
+  AB_CHECK_RC(ab_quantize_rows_e4m3(bf16_ptr(x), reinterpret_cast<uint8_t*>(q.data_ptr()), sx.data_ptr<float>(), M, K,
+                                    x.stride(0), cur_stream()), "ab_quantize_rows_e4m3");
+  g_launches += 1;
+  return {q, sx};
+}
+
+// y = act((xq . wq^T) * sx[m] * sw[n] + bias): xq e4m3 [M, K], sx fp32 [M], wq e4m3 [N, K], sw fp32 [N]
+Tensor gemm_fp8_q(const Tensor& xq, const Tensor& sx, const Tensor& wq, const Tensor& sw, const OptTensor& bias,
+                  int64_t act) {
+  TORCH_CHECK(xq.is_cuda() && xq.scalar_type() == at::kFloat8_e4m3fn && xq.dim() == 2 && xq.is_contiguous(), "gemm_fp8: xq");
+  TORCH_CHECK(wq.is_cuda() && wq.scalar_type() == at::kFloat8_e4m3fn && wq.dim() == 2 && wq.is_contiguous(),
+              "gemm_fp8: w must be contiguous e4m3");
+  const int M = (int)xq.size(0), K = (int)xq.size(1), N = (int)wq.size(0);
+  TORCH_CHECK(wq.size(1) == K && K % 16 == 0 && N % 8 == 0, "gemm_fp8: shapes");
+  TORCH_CHECK(sx.scalar_type() == at::kFloat && sx.is_contiguous() && sx.numel() == M, "gemm_fp8: sx must be fp32 [M]");
+  TORCH_CHECK(sw.scalar_type() == at::kFloat && sw.is_contiguous() && sw.numel() == N, "gemm_fp8: w_scale must be fp32 [N]");
+  if (bias.has_value() && bias->defined())
+    TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->is_contiguous() && bias->numel() == N &&
+                    reinterpret_cast<uintptr_t>(bias->data_ptr()) % 4 == 0,
+                "gemm_fp8: bias must be a contiguous, 4-byte aligned bf16 [N]");
+  c10::cuda::CUDAGuard guard(xq.device());
+  Tensor out = torch::empty({M, N}, xq.options().dtype(at::kBFloat16));
+  AB_CHECK_RC(ab_gemm_fp8(reinterpret_cast<const uint8_t*>(xq.data_ptr()), reinterpret_cast<const uint8_t*>(wq.data_ptr()),
+                          sx.data_ptr<float>(), sw.data_ptr<float>(), bf16_ptr(bias),
+                          reinterpret_cast<__nv_bfloat16*>(out.data_ptr()), M, N, K, N, (int)act, cur_stream()),
+              "ab_gemm_fp8");
+  g_launches += 1;
   return out;
+}
+
+// y = act((quantize_e4m3(x) . w_fp8^T) * sx * sw + bias): x bf16 [M, K], w e4m3 [N, K], w_scale fp32 [N]
+Tensor gemm_fp8(const Tensor& x, const Tensor& w, const Tensor& w_scale, const OptTensor& bias, int64_t act) {
+  check_rows_16b(x, "gemm_fp8");
+  TORCH_CHECK(w.dim() == 2 && w.size(1) == x.size(1), "gemm_fp8: shapes");
+  if (bias.has_value() && bias->defined())   // checked before the quantiser launches
+    TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->numel() == w.size(0), "gemm_fp8: bias must be bf16 [N]");
+  auto qs = quantize_e4m3(x);
+  return gemm_fp8_q(qs[0], qs[1], w, w_scale, bias, act);
 }
 
 // Cross-mesh resharding pack / unpack (pack_sm90.cu): `views` are <= 4-D slices with a contiguous innermost dim; tile k
@@ -743,7 +794,7 @@ void pack_tiles(const std::vector<Tensor>& views, Tensor flat, bool unpack) {
 // Block-scaled MXFP8: e4m3 elements + one UE8M0 scale per 32 K elements, scale atoms of 128 rows x 4 K-blocks
 // (gemm_sm90.cu).  Returns (q [M, K] e4m3, sf uint8 [ceil(M/128), ceil(K/128), 512]).
 std::vector<Tensor> quantize_mxfp8(const Tensor& x) {
-  TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.stride(1) == 1, "quantize_mxfp8: x");
+  check_rows_16b(x, "quantize_mxfp8");
   c10::cuda::CUDAGuard guard(x.device());
   const int M = (int)x.size(0), K = (int)x.size(1);
   TORCH_CHECK(K % 32 == 0, "quantize_mxfp8: K must be a multiple of 32");
@@ -788,7 +839,8 @@ Tensor gemm_mxfp8(const Tensor& x, const Tensor& wq, const Tensor& w_sf, const O
 Tensor gemv_decode(const Tensor& x, const Tensor& w, const OptTensor& w_scale, const OptTensor& bias,
                    const OptTensor& residual, int64_t act, const OptTensor& ln_gamma, const OptTensor& ln_beta,
                    double ln_eps) {
-  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.scalar_type() == at::kBFloat16 && x.stride(1) == 1, "gemv_decode: x");
+  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.scalar_type() == at::kBFloat16 && x.stride(1) == 1 &&
+                  reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0, "gemv_decode: x (16-byte aligned rows)");
   const bool fp8 = w.scalar_type() == at::kFloat8_e4m3fn;
   TORCH_CHECK((fp8 || w.scalar_type() == at::kBFloat16) && w.dim() == 2 && w.is_contiguous() && w.size(1) == x.size(1),
               "gemv_decode: w must be contiguous [N, K] e4m3 / bf16");
@@ -917,6 +969,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("beta2"), py::arg("eps"), py::arg("step"), py::arg("grad_scale"),
         py::arg("clip_coef") = py::none(), py::arg("step_tensor") = py::none());
   m.def("grad_sumsq", &grad_sumsq);
+  m.def("quantize_e4m3", &quantize_e4m3);
+  m.def("gemm_fp8_q", &gemm_fp8_q);
   m.def("gemm_fp8", &gemm_fp8);
   m.def("pack_tiles", &pack_tiles, py::arg("views"), py::arg("flat"), py::arg("unpack") = false);
   m.def("quantize_mxfp8", &quantize_mxfp8);

@@ -203,6 +203,11 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 #pragma unroll
     for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
 
+    float part0[MODE == kModeFp8 ? BLOCK_N / 2 : 1], part1[MODE == kModeFp8 ? BLOCK_N / 2 : 1];  // fp8 scratch
+    auto fold = [&](const float* part) {
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] += part[i];
+    };
     uint32_t prev_stage = 0;
     for (int kb = 0; kb < num_k_blocks; ++kb) {
       mbar_wait(&full_bar[stage], phase);
@@ -226,12 +231,26 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         wgmma_wait<1>();
         if (kb > 0 && tid == 0) mbar_arrive(&empty_bar[prev_stage]);
       } else if constexpr (MODE == kModeFp8) {
-        wgmma_fence();
+        // Hopper's fp8 wgmma accumulates with fewer mantissa bits than fp32, so one chain over all of K loses
+        // precision as K grows.  Each k-block (4 wgmmas, 128 K) goes to a scratch accumulator that is added to acc
+        // in fp32, as CUTLASS's sm90 fp8 mainloop promotes every 4 wgmmas.  Two scratch accumulators alternate so
+        // that one group stays in flight while the previous block is added.
+        auto issue = [&](float* part) {
+          wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < kBlockK / kMmaK; ++k)
-          wgmma_m64n128k32_e4m3(acc, gmma_desc_sw128(sa + k * 32, 16, 1024), gmma_desc_sw128(sb + k * 32, 16, 1024), 1u);
-        wgmma_commit();
-        wgmma_wait<1>();
+          for (int k = 0; k < kBlockK / kMmaK; ++k)
+            wgmma_m64n128k32_e4m3(part, gmma_desc_sw128(sa + k * 32, 16, 1024),
+                                  gmma_desc_sw128(sb + k * 32, 16, 1024), k == 0 ? 0u : 1u);
+          wgmma_commit();
+          wgmma_wait<1>();
+        };
+        if (kb & 1) {
+          issue(part1);
+          fold(part0);
+        } else {
+          issue(part0);
+          if (kb > 0) fold(part1);
+        }
         if (kb > 0 && tid == 0) mbar_arrive(&empty_bar[prev_stage]);
       } else {
         // block-scaled: one K = 32 product per scale block, folded in with sa(row) * sb(col)
@@ -269,6 +288,12 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     if constexpr (MODE != kModeMx) {
       wgmma_wait<0>();
       if (num_k_blocks > 0 && tid == 0) mbar_arrive(&empty_bar[prev_stage]);
+    }
+    if constexpr (MODE == kModeFp8) {
+      if (num_k_blocks & 1)
+        fold(part0);
+      else
+        fold(part1);
     }
 
     // ---- epilogue: fragment j of this thread = rows (row_base, row_base + 8), columns n0 + 8 j + 2 t4 + {0, 1}

@@ -110,6 +110,8 @@ __global__ void __launch_bounds__(kGemvThreads) gemv_decode_kernel(const GemvArg
     const __nv_bfloat16* xrow = a.x + (size_t)m * a.ldx;
     float mean = 0.f, rstd = 1.f;
     if (ln) {
+      // two passes over the row (it stays in L1 / L2), like the stand-alone layer norm: s2/K - mean^2 cancels
+      // catastrophically in fp32 when |mean| >> std
       float s1 = 0.f, s2 = 0.f;
       for (int i = threadIdx.x; i < xchunks; i += kGemvThreads) {
         const int4 v = *reinterpret_cast<const int4*>(xrow + (size_t)i * 8);
@@ -118,13 +120,20 @@ __global__ void __launch_bounds__(kGemvThreads) gemv_decode_kernel(const GemvArg
         for (int q = 0; q < 4; ++q) {
           const float2 f = unpack_bf16x2(u[q]);
           s1 += f.x + f.y;
-          s2 = fmaf(f.x, f.x, fmaf(f.y, f.y, s2));
         }
       }
-      s1 = block_sum(s1, red, warp, lane);
-      s2 = block_sum(s2, red, warp, lane);
-      mean = s1 / (float)K;
-      rstd = rsqrtf(fmaxf(s2 / (float)K - mean * mean, 0.f) + a.ln_eps);
+      mean = block_sum(s1, red, warp, lane) / (float)K;
+      for (int i = threadIdx.x; i < xchunks; i += kGemvThreads) {
+        const int4 v = *reinterpret_cast<const int4*>(xrow + (size_t)i * 8);
+        const uint32_t* u = reinterpret_cast<const uint32_t*>(&v);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const float2 f = unpack_bf16x2(u[q]);
+          const float dx = f.x - mean, dy = f.y - mean;
+          s2 = fmaf(dx, dx, fmaf(dy, dy, s2));
+        }
+      }
+      rstd = rsqrtf(block_sum(s2, red, warp, lane) / (float)K + a.ln_eps);
     }
     auto value8 = [&](int i, float* f) {      // 8 (normalised, bf16-rounded) activations of chunk i
       const int4 v = *reinterpret_cast<const int4*>(xrow + (size_t)i * 8);
@@ -161,7 +170,7 @@ __global__ void __launch_bounds__(kGemvThreads) gemv_decode_kernel(const GemvArg
         for (int q = 0; q < 8; ++q) amax = fmaxf(amax, fabsf(f[q]));
       }
       amax = block_max(amax, red, warp, lane);
-      const float sc = fmaxf(amax, 1e-8f) / 448.f;
+      const float sc = fmaxf(amax, 1e-8f) * (1.f / 448.f);   // quantize_rows_e4m3_kernel's formula, bit for bit
       const float inv = 1.f / sc;
       if (threadIdx.x == 0) xscale[m] = sc;
       for (int i = threadIdx.x; i < xchunks; i += kGemvThreads) {

@@ -809,6 +809,8 @@ def linear_decode(x: Tensor, w: Tensor, w_scale: Optional[Tensor], b: Optional[T
         if ops.native_available() and hasattr(_native(), "gemv_decode") and K % (64 if fp8w else 32) == 0 and \
                 rows * K * (1 if fp8w else 2) <= 200 * 1024:
             x2 = _as2d(x)
+            if x2.stride(0) % 8 or x2.data_ptr() % 16:     # the prologue reads rows 16 bytes at a time
+                x2 = x2.contiguous()
             r2 = None if residual is None else _as2d(residual)
             if ln is not None and ln[0].dtype != torch.bfloat16:
                 x2 = layer_norm(x2, ln[0], ln[1], ln[2])[0]          # the fused prologue reads bf16 gamma / beta
@@ -835,6 +837,8 @@ def linear_fp8(x: Tensor, w_fp8: Tensor, w_scale: Tensor, b: Optional[Tensor] = 
         from alpa_b200 import ops
         if ops.native_available() and hasattr(_native(), "gemm_fp8") and x.shape[-1] % 16 == 0 and w_fp8.shape[0] % 8 == 0:
             x2 = _as2d(x)
+            if x2.stride(0) % 8 or x2.data_ptr() % 16:     # the quantiser reads rows 16 bytes at a time
+                x2 = x2.contiguous()
             y = _native().gemm_fp8(x2, w_fp8, w_scale, b, _ACT_IDS[act])
             return y.view(*x.shape[:-1], w_fp8.shape[0])
     w = (w_fp8.to(torch.float32) * w_scale[:, None]).to(x.dtype)
@@ -930,7 +934,8 @@ def quantize_mxfp8(x: Tensor) -> Tuple[Tensor, Tensor]:
     """x [rows, K] (K % 32 == 0) -> (q e4m3 [rows, K], scale atoms uint8 [ceil(rows/128), ceil(K/128), 512])."""
     assert x.dim() == 2 and x.shape[1] % MX_BLOCK == 0, "quantize_mxfp8: [rows, K] with K % 32 == 0"
     if uses_native(x) and hasattr(_native(), "quantize_mxfp8"):
-        q, sf = _native().quantize_mxfp8(x if x.stride(-1) == 1 else x.contiguous())
+        ok = x.stride(-1) == 1 and x.stride(0) % 8 == 0 and x.data_ptr() % 16 == 0
+        q, sf = _native().quantize_mxfp8(x if ok else x.contiguous())
         return q, sf
     return _quantize_mxfp8_ref(x)
 
@@ -949,7 +954,9 @@ def linear_mxfp8(x: Tensor, w_q: Tensor, w_sf: Tensor, b: Optional[Tensor] = Non
     K, N = x.shape[-1], w_q.shape[0]
     x2 = _as2d(x)
     if uses_native(x) and hasattr(_native(), "gemm_mxfp8") and K % MX_BLOCK == 0 and N % 8 == 0:
-        y = _native().gemm_mxfp8(x2 if x2.stride(-1) == 1 else x2.contiguous(), w_q, w_sf, b, _ACT_IDS[act])
+        if x2.stride(0) % 8 or x2.data_ptr() % 16:         # the quantiser reads rows 16 bytes at a time
+            x2 = x2.contiguous()
+        y = _native().gemm_mxfp8(x2, w_q, w_sf, b, _ACT_IDS[act])
         return y.view(*x.shape[:-1], N)
     xq, x_sf = _quantize_mxfp8_ref(x2)
     y = F.linear(dequantize_mxfp8(xq, x_sf), dequantize_mxfp8(w_q, w_sf), None if b is None else b.float())
