@@ -26,6 +26,7 @@ many k-blocks, both tile widths and all operand majors, batches with padded batc
 buffers (a read outside the matrix poisons the result) and outputs inside sentinel-filled buffers (a write outside
 the view changes the sentinel).
 """
+import itertools
 import math
 import os
 import sys
@@ -571,7 +572,7 @@ def test_bf16_gemm_wgrad_k16384(M, N):
 # GPU: bf16 GEMM epilogues
 # ---------------------------------------------------------------------------------------------------------------------
 EPILOGUES = ["bias", "bias_gelu_aux", "bias_relu", "residual", "bias_residual", "dgelu", "drelu", "alpha_bias",
-             "out_fp32", "acc_fp32", "acc_bf16", "acc_residual"]
+             "out_fp32", "acc_fp32", "acc_bf16", "acc_residual", "alpha_out_fp32"]
 # (M, N, K, batch, trans_a, trans_b, block_n): tails on both tile widths, the dgrad layout (B MN-major), a batch
 EPI_CONFIGS = [
     (129, 1000, 264, None, False, True, 128),
@@ -595,7 +596,7 @@ def test_bf16_gemm_epilogue(epi, cfg):
     C = _native()
     ck = Checker()
     M, N, K, batch, ta, tb, bn = cfg
-    fp32 = epi in ("out_fp32", "acc_fp32", "acc_residual")
+    fp32 = epi in ("out_fp32", "acc_fp32", "acc_residual", "alpha_out_fp32")
     seed = 100 * EPI_CONFIGS.index(cfg) + EPILOGUES.index(epi)
     a, b, sa, sb = _operands_gpu(M, N, K, ta, tb, 2000 + seed, batch=batch, mean=1.0 if fp32 else 0.0)
     g = _gen(3000 + seed, "cuda")
@@ -607,7 +608,7 @@ def test_bf16_gemm_epilogue(epi, cfg):
     aux_in = Sentinel(shape, BF16, aux_in_values(M, N, g, "cuda", batch)) if epi in ("dgelu", "drelu") else None
     aux_out = Sentinel(shape, BF16) if epi == "bias_gelu_aux" else None
     act = {"bias_gelu_aux": ACT_GELU, "bias_relu": ACT_RELU, "dgelu": ACT_DGELU, "drelu": ACT_DRELU}.get(epi, ACT_NONE)
-    alpha = 0.37 if epi == "alpha_bias" else 1.0
+    alpha = 0.37 if epi.startswith("alpha") else 1.0
     old = None
     if epi == "acc_bf16":                                    # a partial sum of the same size as this product
         old = torch.randn(shape, generator=g, device="cuda").to(BF16)
@@ -644,6 +645,10 @@ def test_bf16_gemm_epilogue(epi, cfg):
 FP8_K = [16, 48, 528, 2560, 10240]
 FP8_N = [8, 72, 2560]
 FP8_M = [1, 130, 257]
+# (M, N, K): every K x N of the grid with M cycling through FP8_M, then a serving shape of 16 x 80 tiles, more than
+# there are SMs, so that each CTA of the persistent kernel runs several tiles
+FP8_SHAPES = [(FP8_M[i % 3], N, K) for i, (K, N) in enumerate(itertools.product(FP8_K, FP8_N))]
+FP8_SHAPES.append((2048, 10240, 2560))
 
 
 def _fp8_x(M, K, g):
@@ -680,27 +685,23 @@ def test_e4m3_quantiser():
 def test_fp8_gemm():
     C = _native()
     ck = Checker()
-    i = 0
-    for K in FP8_K:
-        for N in FP8_N:
-            M = FP8_M[i % 3]
-            act = (ACT_NONE, ACT_RELU, ACT_GELU)[i % 3]
-            use_bias = i % 2 == 0
-            i += 1
-            g = _gen(400 + i, "cuda")
-            x = _fp8_x(M, K, g)
-            wq, sw = _fp8_w(N, K, g)
-            bias = (torch.randn(N, generator=g, device="cuda") * 0.1).to(BF16) if use_bias else None
-            q, sx = C.quantize_e4m3(x)
-            y = C.gemm_fp8_q(q, sx, wq, sw, bias, act)
-            ref = (q.to(F64) @ wq.to(F64).t()) * sx.to(F64)[:, None] * sw.to(F64)[None, :]
-            if bias is not None:
-                ref = ref + bias.to(F64)
-            ref = act64(ref, act)
-            key = f"gemm fp8 K{K}"
-            ck.bf16(key, f"gemm fp8 M{M} N{N} K{K} act{act} bias={use_bias}", y, ref, _bf(ref))
-            y2 = C.gemm_fp8(x, wq, sw, bias, act)
-            ck.require(torch.equal(y, y2), f"gemm_fp8 M{M} N{N} K{K}: differs from quantize_e4m3 + gemm_fp8_q")
+    for i, (M, N, K) in enumerate(FP8_SHAPES):
+        act = (ACT_NONE, ACT_RELU, ACT_GELU)[i % 3]
+        use_bias = i % 2 == 0
+        g = _gen(401 + i, "cuda")
+        x = _fp8_x(M, K, g)
+        wq, sw = _fp8_w(N, K, g)
+        bias = (torch.randn(N, generator=g, device="cuda") * 0.1).to(BF16) if use_bias else None
+        q, sx = C.quantize_e4m3(x)
+        y = C.gemm_fp8_q(q, sx, wq, sw, bias, act)
+        ref = (q.to(F64) @ wq.to(F64).t()) * sx.to(F64)[:, None] * sw.to(F64)[None, :]
+        if bias is not None:
+            ref = ref + bias.to(F64)
+        ref = act64(ref, act)
+        key = f"gemm fp8 K{K}"
+        ck.bf16(key, f"gemm fp8 M{M} N{N} K{K} act{act} bias={use_bias}", y, ref, _bf(ref))
+        y2 = C.gemm_fp8(x, wq, sw, bias, act)
+        ck.require(torch.equal(y, y2), f"gemm_fp8 M{M} N{N} K{K}: differs from quantize_e4m3 + gemm_fp8_q")
     _report(ck)
 
 
@@ -729,31 +730,32 @@ def test_mxfp8_quantiser_bit_exact(M, K):
         f"{int((q.cpu().view(torch.uint8) != rq.view(torch.uint8)).sum())} e4m3 bytes differ"
 
 
+# (M, N, K): every K x N of the grid with M cycling through 1, 130, 257, then 8 x 20 tiles, more than there are SMs
+MX_SHAPES = [((1, 130, 257)[i % 3], N, K) for i, (K, N) in enumerate(itertools.product((32, 96, 160, 2560, 10240), (8, 72)))]
+MX_SHAPES.append((1024, 2560, 2560))
+
+
 @pytest.mark.gpu
 def test_mxfp8_gemm():
     from alpa_b200.ops import primitives as P
     C = _native()
     ck = Checker()
-    i = 0
-    for K in (32, 96, 160, 2560, 10240):
-        for N in (8, 72):
-            M = (1, 130, 257)[i % 3]
-            act = (ACT_NONE, ACT_RELU, ACT_GELU)[i % 3]
-            use_bias = i % 2 == 1
-            i += 1
-            g = _gen(600 + i, "cuda")
-            x = mx_operand(M, K, g, "cuda")
-            w = mx_operand(N, K, g, "cuda")
-            wq, wsf = (t.cuda() for t in P._quantize_mxfp8_ref(w.cpu()))
-            bias = (torch.randn(N, generator=g, device="cuda") * 0.1).to(BF16) if use_bias else None
-            q, sf = C.quantize_mxfp8(x)
-            y = C.gemm_mxfp8_q(q, sf, wq, wsf, bias, act)
-            ref = mx_dequant64(q, sf) @ mx_dequant64(wq, wsf).t()
-            if bias is not None:
-                ref = ref + bias.to(F64)
-            ref = act64(ref, act)
-            key = f"gemm mxfp8 K{K}"
-            ck.bf16(key, f"gemm mxfp8 M{M} N{N} K{K} act{act} bias={use_bias}", y, ref, _bf(ref))
+    for i, (M, N, K) in enumerate(MX_SHAPES):
+        act = (ACT_NONE, ACT_RELU, ACT_GELU)[i % 3]
+        use_bias = i % 2 == 1
+        g = _gen(601 + i, "cuda")
+        x = mx_operand(M, K, g, "cuda")
+        w = mx_operand(N, K, g, "cuda")
+        wq, wsf = (t.cuda() for t in P._quantize_mxfp8_ref(w.cpu()))
+        bias = (torch.randn(N, generator=g, device="cuda") * 0.1).to(BF16) if use_bias else None
+        q, sf = C.quantize_mxfp8(x)
+        y = C.gemm_mxfp8_q(q, sf, wq, wsf, bias, act)
+        ref = mx_dequant64(q, sf) @ mx_dequant64(wq, wsf).t()
+        if bias is not None:
+            ref = ref + bias.to(F64)
+        ref = act64(ref, act)
+        key = f"gemm mxfp8 K{K}"
+        ck.bf16(key, f"gemm mxfp8 M{M} N{N} K{K} act{act} bias={use_bias}", y, ref, _bf(ref))
     _report(ck)
 
 

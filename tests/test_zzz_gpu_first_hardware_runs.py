@@ -39,17 +39,11 @@ def _run_inner(script, timeout, *args):
     print(r.stderr[-2000:])
     # the result lines go to pytest's warnings summary: it is printed even for xpassed / xfailed tests under -q, so the
     # numbers of the first hardware run end up in the session log either way
-    keep = [ln.strip() for ln in r.stdout.splitlines() if ln.startswith(("mxfp8", "native comm", "p2p", "cached pipeshard", "attention_cached", "train feature", "pack ", "BENCH "))]
+    keep = [ln.strip() for ln in r.stdout.splitlines() if ln.startswith(("native comm", "p2p", "cached pipeshard", "attention_cached", "train feature", "pack ", "BENCH "))]
     if r.returncode != 0:
         keep += ["rc=%d" % r.returncode] + [ln.strip() for ln in r.stderr.splitlines()[-6:]]
     warnings.warn("first hardware run of %s: %s" % (script, " | ".join(keep)[-1800:]))
     return r
-
-
-@pytest.mark.xfail(strict=False, reason="block-scaled MXFP8 GEMM (wgmma, scales folded per K block): first hardware run")
-def test_mxfp8_block_scaled_gemm_first_hardware_run():
-    r = _run("gpu_check_mxfp8.py", 150)
-    assert r.returncode == 0 and "mxfp8 check: ok" in r.stdout
 
 
 @pytest.mark.xfail(strict=False, reason="native communication module (dlopen'ed NCCL / CUDA runtime): first hardware run")
@@ -84,8 +78,8 @@ def test_resharding_pack_kernel_first_hardware_run():
 
 @pytest.mark.xfail(strict=False, reason="informational: GEMM / attention timings of the kernels at HEAD on this box")
 def test_kernel_timings_at_head():
-    """Not a validation (the numerics of these kernels are checked by tests/test_gpu_kernels.py): re-runs the timing
-    sections of the GPU check scripts so that the session log carries TFLOPS of the wgmma GEMM (against cuBLAS) and of
-    the attention forward / backward as built from this commit."""
+    """Not a validation (the numerics of these kernels are checked by tests/test_gemm_numerics.py and
+    tests/test_kernel_numerics.py): runs the timing sections of scripts/gpu_check.py so that the session log carries
+    TFLOPS of the wgmma GEMM (against cuBLAS) and of the attention forward / backward as built from this commit."""
     r = _run("gpu_check.py", 240, "gemm_bench", "attn")
     assert r.returncode == 0
