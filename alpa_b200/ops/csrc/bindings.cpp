@@ -35,8 +35,9 @@ static std::atomic<long long> g_launches{0};
 Tensor gemm(const Tensor& a, const Tensor& b, bool trans_a, bool trans_b, const OptTensor& out_opt,
             const OptTensor& bias, const OptTensor& residual, const OptTensor& aux_out,
             const OptTensor& aux_in, int64_t act, double alpha, bool accumulate, bool out_fp32,
-            int64_t block_n) {
+            int64_t block_n, const std::string& epilogue) {
   TORCH_CHECK(a.is_cuda() && b.is_cuda(), "gemm: CUDA tensors required");
+  TORCH_CHECK(epilogue == "auto" || epilogue == "generic", "gemm: epilogue must be 'auto' or 'generic'");
   TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16, "gemm: bf16 only");
   TORCH_CHECK(a.dim() == b.dim() && (a.dim() == 2 || a.dim() == 3), "gemm: 2-D or 3-D operands");
   c10::cuda::CUDAGuard guard(a.device());
@@ -63,6 +64,7 @@ Tensor gemm(const Tensor& a, const Tensor& b, bool trans_a, bool trans_b, const 
   g.a = a.data_ptr();
   g.b = b.data_ptr();
   g.block_n = (int)block_n;
+  g.epilogue_generic = epilogue == "generic" ? 1 : 0;
 
   Tensor out;
   if (out_opt.has_value() && out_opt->defined()) {
@@ -935,7 +937,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("trans_b") = false, py::arg("out") = py::none(), py::arg("bias") = py::none(),
         py::arg("residual") = py::none(), py::arg("aux_out") = py::none(),
         py::arg("aux_in") = py::none(), py::arg("act") = 0, py::arg("alpha") = 1.0,
-        py::arg("accumulate") = false, py::arg("out_fp32") = false, py::arg("block_n") = 0);
+        py::arg("accumulate") = false, py::arg("out_fp32") = false, py::arg("block_n") = 0,
+        py::arg("epilogue") = "auto");
   m.def("gemm_scatter", &gemm_scatter, py::arg("a"), py::arg("b"), py::arg("trans_b"), py::arg("peer_ptrs"),
         py::arg("flag_ptrs"), py::arg("slot"), py::arg("rows_per_dst"), py::arg("ldc"), py::arg("m_block_rotate"),
         py::arg("max_ctas"), py::arg("trans_a") = false);

@@ -1,5 +1,6 @@
 // alpa_b200 GEMMs for sm_90a: persistent, warp-specialised, TMA -> smem ring -> wgmma.mma_async (accumulators in the
-// registers of two consumer warpgroups) -> register epilogue.
+// registers of two consumer warpgroups) -> epilogue (bf16: staged in shared memory and TMA-stored for the training
+// step's epilogue kinds, register stores for everything else; see kEpi*).
 //
 // Replaces the reference's cuBLAS custom-call path (XLA/service/gpu/matmul_utils.cc:438-480) for
 // K1/K3/K4/K5/K8/K13 of SURVEY.md §2.5.
@@ -42,13 +43,35 @@ constexpr int kGroupM = 16;  // M-blocks per band of the tile order (see tile_co
 enum : uint32_t { kMajorK = 0, kMajorMN = 1 };  // operand major (wgmma transpose flag)
 enum : int { kModeBf16 = 0, kModeFp8 = 1, kModeMx = 2 };
 
-template <int BLOCK_N>
+// bf16 epilogue kinds.  Each is its own instantiation, so the fully unrolled fragment loop holds only the work of one
+// kind.  The fast kinds (all but kEpiGeneric) stage the bf16 tile in shared memory and write it with TMA stores; they
+// need alpha == 1, a bf16 output without accumulate or residual, and output / aux tensors a TMA map can describe.
+// kEpiGeneric keeps every runtime option (alpha, residual, fp32 output, accumulate, peer scatter, odd row strides)
+// and stores from registers.
+enum : int {
+  kEpiGeneric = 0,
+  kEpiStore = 1,        // out = acc
+  kEpiBias = 2,         // out = acc + bias
+  kEpiBiasGeluAux = 3,  // aux_out = acc + bias, out = gelu(aux_out)
+  kEpiDGelu = 4,        // out = acc * gelu'(aux_in)
+};
+
+template <int BLOCK_N, int EPI>
 struct SmemLayout {
   static constexpr int kABytes = BLOCK_M * kRowBytes;  // 16 KB
   static constexpr int kBBytes = BLOCK_N * kRowBytes;
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStages = (BLOCK_N == 256) ? 4 : 6;
-  static constexpr int kTotal = kStages * kStageBytes + 1024 /*barriers*/ + 1024 /*align slack*/;
+  // Fast epilogue kinds: each consumer warpgroup owns two 64 x 64 bf16 chunk buffers (128-byte rows, 128-byte
+  // swizzle), so it fills one while the TMA store of the other reads it, and a copy of the tile's bias slice.  The
+  // generic epilogue reserves neither: shared memory it does not use is left to the L1 cache, which the fp8 and
+  // MXFP8 epilogues read their scales through.
+  static constexpr int kChunkBytes = 64 * 64 * 2;
+  static constexpr int kStagingBytes = EPI == kEpiGeneric ? 0 : 2 * 2 * kChunkBytes;
+  static constexpr int kBiasBytes = EPI == kEpiGeneric ? 0 : 2 * BLOCK_N * 2;
+  static constexpr int kTotal = kStages * kStageBytes + kStagingBytes + 1024 /*barriers*/ + kBiasBytes +
+                                1024 /*align slack*/;
+  static_assert(kTotal <= 232448, "exceeds the 227 KB of shared memory per block");
 };
 
 // fp8 / mxfp8 epilogue and scale operands
@@ -88,22 +111,30 @@ __device__ __forceinline__ float mx_scale(const uint8_t* sf, int num_k_atoms, in
   return e == 0 ? ldexpf(1.f, -127) : __uint_as_float((uint32_t)e << 23);
 }
 
-template <int BLOCK_N, int MODE, uint32_t A_MAJOR, uint32_t B_MAJOR>
+// tmap_c / tmap_aux (fast epilogue kinds only): the bf16 output and aux_out or aux_in as (N, M, batch) maps with
+// 64 x 64 boxes.  The extents are exact, so TMA clips the M and N tails of a tile.
+template <int BLOCK_N, int MODE, uint32_t A_MAJOR, uint32_t B_MAJOR, int EPI>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                 const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_aux,
                  const GemmEpilogue ep, const Fp8Params fp, int M, int N, int K, int batch) {
-  using L = SmemLayout<BLOCK_N>;
+  using L = SmemLayout<BLOCK_N, EPI>;
   constexpr int kStages = L::kStages;
   constexpr int kElemBytes = MODE == kModeBf16 ? 2 : 1;
   constexpr int kBlockK = kRowBytes / kElemBytes;
   constexpr int kMmaK = 32 / kElemBytes;  // K per wgmma: 16 bf16 / 32 e4m3 (32 bytes either way)
+  static_assert(EPI == kEpiGeneric || MODE == kModeBf16, "fast epilogue kinds are bf16 only");
+  constexpr bool kHasBias = EPI == kEpiBias || EPI == kEpiBiasGeluAux;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + kStages * L::kABytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * L::kStageBytes);
+  uint8_t* smem_out = smem + kStages * L::kStageBytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_out + L::kStagingBytes);
   uint64_t* empty_bar = full_bar + kStages;
+  uint64_t* aux_bar = empty_bar + kStages;  // [2 consumer warpgroups][2 chunk buffers]: aux_in loads
+  uint32_t* bias_smem = reinterpret_cast<uint32_t*>(smem_out + L::kStagingBytes + 1024);  // [2][BLOCK_N / 2] pairs
 
   const int wg = threadIdx.x >> 7;
   const int num_m_blocks = (M + BLOCK_M - 1) / BLOCK_M;
@@ -118,6 +149,9 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 2);  // one arrival per consumer warpgroup
+    }
+    if constexpr (EPI == kEpiDGelu) {
+      for (int i = 0; i < 4; ++i) mbar_init(&aux_bar[i], 1);
     }
     mbar_fence_init();
   }
@@ -195,11 +229,37 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const int g = lane >> 2, t4 = lane & 3;
   uint32_t stage = 0, phase = 0;
   float acc[BLOCK_N / 2];
+  // fast epilogue state of this warpgroup: its two staging buffers, its aux_in barriers and bias slice, the number
+  // of TMA stores it has issued (they alternate between the buffers) and the parities of its aux_in barriers
+  uint8_t* const stage_out = smem_out + cw * (2 * L::kChunkBytes);
+  uint64_t* const aux_bar_wg = aux_bar + 2 * cw;
+  uint32_t* const bias_wg = bias_smem + cw * (BLOCK_N / 2);
+  uint32_t store_count = 0, aux_phase = 0;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     int b, m_blk, n_blk;
     tile_coords(tile, b, m_blk, n_blk);
     const int row_base = m_blk * BLOCK_M + cw * 64 + wi * 16 + g;  // + 8 for the second row of a fragment
     const int n0 = n_blk * BLOCK_N;
+    const int m0w = m_blk * BLOCK_M + cw * 64;  // first row of this warpgroup
+    const int n_chunks = m0w < M ? min(BLOCK_N / 64, (N - n0 + 63) / 64) : 0;  // 64-column chunks with data
+    // Epilogue operands are fetched before the mainloop, so their latency hides behind it: the tile's bias slice by
+    // cp.async into this warpgroup's copy (its readers passed the previous tile's last wg_barrier), and aux_in's first
+    // two 64-column chunks by TMA into the staging buffers (once the previous tile's stores have finished reading them).
+    if constexpr (kHasBias) {
+      if (tid < BLOCK_N / 2 && n0 + 2 * tid < N)
+        asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"(smem_u32(bias_wg + tid)),
+                     "l"(ep.bias + n0 + 2 * tid)
+                     : "memory");
+    }
+    if constexpr (EPI == kEpiDGelu) {
+      if (tid == 0) {
+        tma_store_wait_read<0>();
+        for (int c = 0; c < 2 && c < n_chunks; ++c) {
+          mbar_expect_tx(&aux_bar_wg[c], L::kChunkBytes);
+          tma_load_3d(stage_out + c * L::kChunkBytes, &tmap_aux, &aux_bar_wg[c], n0 + 64 * c, m0w, b);
+        }
+      }
+    }
 #pragma unroll
     for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
 
@@ -297,7 +357,112 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     }
 
     // ---- epilogue: fragment j of this thread = rows (row_base, row_base + 8), columns n0 + 8 j + 2 t4 + {0, 1}
-    if constexpr (MODE == kModeBf16) {
+    if constexpr (EPI != kEpiGeneric) {
+      // Chunk c = columns [64 c, 64 c + 64) of the warpgroup's 64 rows.  In a 128-byte-swizzled 64 x 64 bf16 buffer,
+      // element (r, col) sits at byte r * 128 + ((col / 8) ^ (r % 8)) * 16 + (col % 8) * 2; fragment row r = 16 wi +
+      // g + 8 hi has r % 8 == g, and the 32 lanes of a warp hit 32 different banks.
+      auto frag_off = [&](int jj, int hi) -> uint32_t {
+        return (wi * 16 + g + 8 * hi) * 128 + ((jj ^ g) << 4) + t4 * 4;
+      };
+      if constexpr (kHasBias) {
+        asm volatile("cp.async.wait_all;\n" ::: "memory");  // read after the first wg_barrier of the chunk loop
+      }
+      // Stage one chunk (value(j, hi) -> bf16x2 of fragment j, row half hi) and TMA-store it.  Before a buffer is
+      // refilled, only the read of the store issued from it two stores earlier must be complete; the writes to
+      // global memory stay in flight into the next tile's mainloop.
+      auto store_chunk = [&](const CUtensorMap* map, int c, auto&& value) {
+        uint8_t* buf = stage_out + (store_count & 1) * L::kChunkBytes;
+        const uint32_t sbuf = smem_u32(buf);
+        if (tid == 0) tma_store_wait_read<1>();
+        wg_barrier(1 + cw);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+          for (int hi = 0; hi < 2; ++hi) {
+            const uint32_t v = value(8 * c + jj, hi);
+            asm volatile("st.shared.b32 [%0], %1;\n" ::"r"(sbuf + frag_off(jj, hi)), "r"(v) : "memory");
+          }
+        }
+        fence_proxy_async_smem();
+        wg_barrier(1 + cw);
+        if (tid == 0) {
+          tma_store_3d(map, buf, n0 + 64 * c, m0w, b);
+          tma_store_commit();
+        }
+        ++store_count;
+      };
+      auto biased = [&](int j, int hi) {
+        const float2 f = unpack_bf16x2(bias_wg[4 * j + t4]);
+        return make_float2(acc[4 * j + 2 * hi] + f.x, acc[4 * j + 2 * hi + 1] + f.y);
+      };
+#pragma unroll
+      for (int c = 0; c < BLOCK_N / 64; ++c) {
+        if (c >= n_chunks) break;
+        if constexpr (EPI == kEpiStore) {
+          store_chunk(&tmap_c, c, [&](int j, int hi) { return pack_bf16x2(acc[4 * j + 2 * hi], acc[4 * j + 2 * hi + 1]); });
+        } else if constexpr (EPI == kEpiBias) {
+          store_chunk(&tmap_c, c, [&](int j, int hi) {
+            const float2 v = biased(j, hi);
+            return pack_bf16x2(v.x, v.y);
+          });
+        } else if constexpr (EPI == kEpiBiasGeluAux) {
+          // the pre-activation (saved for GELU backward) and the output, staged in one pass: one buffer each
+          const uint32_t s_aux = smem_u32(stage_out), s_out = smem_u32(stage_out + L::kChunkBytes);
+          if (tid == 0) tma_store_wait_read<0>();
+          wg_barrier(1 + cw);
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+            for (int hi = 0; hi < 2; ++hi) {
+              const float2 v = biased(8 * c + jj, hi);
+              asm volatile("st.shared.b32 [%0], %1;\n" ::"r"(s_aux + frag_off(jj, hi)), "r"(pack_bf16x2(v.x, v.y))
+                           : "memory");
+              asm volatile("st.shared.b32 [%0], %1;\n" ::"r"(s_out + frag_off(jj, hi)),
+                           "r"(pack_bf16x2(gelu_erf(v.x), gelu_erf(v.y)))
+                           : "memory");
+            }
+          }
+          fence_proxy_async_smem();
+          wg_barrier(1 + cw);
+          if (tid == 0) {
+            tma_store_3d(&tmap_aux, stage_out, n0 + 64 * c, m0w, b);
+            tma_store_3d(&tmap_c, stage_out + L::kChunkBytes, n0 + 64 * c, m0w, b);
+            tma_store_commit();
+          }
+        } else {
+          // kEpiDGelu: chunk c's aux_in was loaded into buffer c % 2; the result overwrites it in place and is
+          // stored from there.  Chunk c + 2 is then loaded into the same buffer once that store has read it.
+          const int bi = c & 1;
+          uint8_t* buf = stage_out + bi * L::kChunkBytes;
+          const uint32_t sbuf = smem_u32(buf);
+          mbar_wait(&aux_bar_wg[bi], (aux_phase >> bi) & 1);
+          aux_phase ^= 1u << bi;
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+            for (int hi = 0; hi < 2; ++hi) {
+              const int j = 8 * c + jj;
+              uint32_t zb;
+              asm volatile("ld.shared.b32 %0, [%1];\n" : "=r"(zb) : "r"(sbuf + frag_off(jj, hi)) : "memory");
+              const float2 z = unpack_bf16x2(zb);
+              const uint32_t v = pack_bf16x2(acc[4 * j + 2 * hi] * dgelu_erf(z.x), acc[4 * j + 2 * hi + 1] * dgelu_erf(z.y));
+              asm volatile("st.shared.b32 [%0], %1;\n" ::"r"(sbuf + frag_off(jj, hi)), "r"(v) : "memory");
+            }
+          }
+          fence_proxy_async_smem();
+          wg_barrier(1 + cw);
+          if (tid == 0) {
+            tma_store_3d(&tmap_c, buf, n0 + 64 * c, m0w, b);
+            tma_store_commit();
+            if (c + 2 < n_chunks) {
+              tma_store_wait_read<0>();
+              mbar_expect_tx(&aux_bar_wg[bi], L::kChunkBytes);
+              tma_load_3d(buf, &tmap_aux, &aux_bar_wg[bi], n0 + 64 * (c + 2), m0w, b);
+            }
+          }
+        }
+      }
+    } else if constexpr (MODE == kModeBf16) {
 #pragma unroll
       for (int hi = 0; hi < 2; ++hi) {
         const int row = row_base + 8 * hi;
@@ -413,6 +578,9 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         }
       }
     }
+  }
+  if constexpr (EPI != kEpiGeneric) {
+    if (tid == 0) tma_store_wait<0>();  // the staging buffers must outlive the stores that read them
   }
 }
 
@@ -586,11 +754,12 @@ int num_sms() {
   return g_num_sms;
 }
 
-template <int BLOCK_N, int MODE, uint32_t A_MAJOR, uint32_t B_MAJOR>
-static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, const Fp8Params& fp, int M,
-                  int N, int K, int batch, int max_ctas, cudaStream_t stream) {
-  auto kern = gemm_sm90_kernel<BLOCK_N, MODE, A_MAJOR, B_MAJOR>;
-  constexpr int smem = SmemLayout<BLOCK_N>::kTotal;
+template <int BLOCK_N, int MODE, uint32_t A_MAJOR, uint32_t B_MAJOR, int EPI>
+static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const CUtensorMap& taux,
+                  const GemmEpilogue& ep, const Fp8Params& fp, int M, int N, int K, int batch, int max_ctas,
+                  cudaStream_t stream) {
+  auto kern = gemm_sm90_kernel<BLOCK_N, MODE, A_MAJOR, B_MAJOR, EPI>;
+  constexpr int smem = SmemLayout<BLOCK_N, EPI>::kTotal;
   static bool attr_set = false;
   if (!attr_set) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
@@ -600,14 +769,36 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilog
   const int tiles = ((M + BLOCK_M - 1) / BLOCK_M) * ((N + BLOCK_N - 1) / BLOCK_N) * batch;
   int grid = tiles < num_sms() ? tiles : num_sms();
   if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
-  kern<<<grid, kNumThreads, smem, stream>>>(ta, tb, ep, fp, M, N, K, batch);
+  kern<<<grid, kNumThreads, smem, stream>>>(ta, tb, tc, taux, ep, fp, M, N, K, batch);
   return cudaGetLastError() == cudaSuccess ? 0 : 400;
+}
+
+// The epilogue kind a bf16 GEMM runs with.  Only the kinds the training step uses are instantiated for each operand
+// major combination: the plain store for all four, bias and bias + GELU + aux_out for the forward (K, K) and dGELU
+// for the dgrad (K, MN).  Everything else takes the generic epilogue.
+static int epilogue_kind(const GemmArgs& g) {
+  const GemmEpilogue& e = g.ep;
+  auto tma_ok = [](const void* p) { return p != nullptr && (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  if (g.epilogue_generic || e.scatter_rows_per_dst > 0 || e.a_ready != nullptr || e.out_fp32 || e.accumulate ||
+      e.alpha != 1.0f || e.residual != nullptr || !tma_ok(e.out) || e.ldc % 8 != 0 ||
+      (g.batch > 1 && e.batch_stride_c % 8 != 0))
+    return kEpiGeneric;
+  const bool fwd = g.a_major == kMajorK && g.b_major == kMajorK;
+  const bool dgrad = g.a_major == kMajorK && g.b_major == kMajorMN;
+  if (e.aux_in == nullptr && e.aux_out == nullptr) {
+    if (e.act == kActNone) return e.bias == nullptr ? kEpiStore : (fwd ? kEpiBias : kEpiGeneric);
+    return kEpiGeneric;
+  }
+  if (fwd && e.bias != nullptr && e.act == kActGelu && e.aux_in == nullptr && tma_ok(e.aux_out))
+    return kEpiBiasGeluAux;
+  if (dgrad && e.bias == nullptr && e.act == kActDGelu && e.aux_out == nullptr && tma_ok(e.aux_in)) return kEpiDGelu;
+  return kEpiGeneric;
 }
 
 template <int BLOCK_N, uint32_t A_MAJOR, uint32_t B_MAJOR>
 static int launch_bf16(const GemmArgs& g, cudaStream_t stream) {
   constexpr int BK = kRowBytes / 2;
-  CUtensorMap ta, tb;
+  CUtensorMap ta, tb, tc{}, taux{};
   int rc;
   if (A_MAJOR == kMajorK)
     rc = make_tmap_bf16_3d(&ta, g.a, g.K, g.M, g.batch, g.lda, g.batch_stride_a, BK, BLOCK_M);
@@ -619,16 +810,40 @@ static int launch_bf16(const GemmArgs& g, cudaStream_t stream) {
   else
     rc = make_tmap_bf16_3d(&tb, g.b, g.N, g.K, g.batch, g.ldb, g.batch_stride_b, 64, BK);
   if (rc) return 200 + rc;
-  return launch<BLOCK_N, kModeBf16, A_MAJOR, B_MAJOR>(ta, tb, g.ep, Fp8Params{}, g.M, g.N, g.K, g.batch, g.max_ctas,
-                                                      stream);
+  int kind = epilogue_kind(g);
+  if (kind != kEpiGeneric) {
+    // a layout the tensor-map encoder rejects is written by the generic epilogue instead
+    const void* aux = kind == kEpiBiasGeluAux ? static_cast<const void*>(g.ep.aux_out)
+                      : kind == kEpiDGelu     ? static_cast<const void*>(g.ep.aux_in)
+                                              : nullptr;
+    if (make_tmap_bf16_3d(&tc, g.ep.out, g.N, g.M, g.batch, g.ep.ldc, g.ep.batch_stride_c, 64, 64) ||
+        (aux != nullptr && make_tmap_bf16_3d(&taux, aux, g.N, g.M, g.batch, g.ep.ldc, g.ep.batch_stride_c, 64, 64)))
+      kind = kEpiGeneric;
+  }
+#define AB_LAUNCH(EPI)                                                                                      \
+  return launch<BLOCK_N, kModeBf16, A_MAJOR, B_MAJOR, EPI>(ta, tb, tc, taux, g.ep, Fp8Params{}, g.M, g.N, g.K, \
+                                                           g.batch, g.max_ctas, stream)
+  constexpr bool kFwd = A_MAJOR == kMajorK && B_MAJOR == kMajorK;
+  constexpr bool kDgrad = A_MAJOR == kMajorK && B_MAJOR == kMajorMN;
+  if (kind == kEpiStore) AB_LAUNCH(kEpiStore);
+  if constexpr (kFwd) {
+    if (kind == kEpiBias) AB_LAUNCH(kEpiBias);
+    if (kind == kEpiBiasGeluAux) AB_LAUNCH(kEpiBiasGeluAux);
+  }
+  if constexpr (kDgrad) {
+    if (kind == kEpiDGelu) AB_LAUNCH(kEpiDGelu);
+  }
+  AB_LAUNCH(kEpiGeneric);
+#undef AB_LAUNCH
 }
 
 template <int MODE>
 static int launch_fp8(const uint8_t* a, const uint8_t* b, const Fp8Params& fp, int M, int N, int K, cudaStream_t st) {
-  CUtensorMap ta, tb;
+  CUtensorMap ta, tb, unused{};
   if (make_tmap_3d(&ta, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, a, K, M, 1, K, 0, kRowBytes, BLOCK_M)) return 100;
   if (make_tmap_3d(&tb, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, b, K, N, 1, K, 0, kRowBytes, 128)) return 200;
-  return launch<128, MODE, kMajorK, kMajorK>(ta, tb, GemmEpilogue{}, fp, M, N, K, 1, 0, st);
+  return launch<128, MODE, kMajorK, kMajorK, kEpiGeneric>(ta, tb, unused, unused, GemmEpilogue{}, fp, M, N, K, 1, 0,
+                                                          st);
 }
 
 }  // namespace ab

@@ -50,6 +50,7 @@ struct GemmArgs {
   long long batch_stride_a = 0, batch_stride_b = 0;
   int block_n = 0;               // 0 = auto, 128 or 256
   int max_ctas = 0;              // 0 = all SMs (fused comm kernels reserve SMs)
+  int epilogue_generic = 0;      // 1 = always the generic (register-store) epilogue, for comparing it with the others
   GemmEpilogue ep;
 };
 

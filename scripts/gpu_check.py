@@ -1,7 +1,8 @@
 """Kernel timings on the GPU: one section per kernel group, each printing `BENCH` lines (CUDA events, median of 20
 calls after 5 warm-ups).  The kernels' numerics are checked by the GPU tests under tests/.
 
-usage: python scripts/gpu_check.py [section ...]    sections: gemm_bench misc attn moe fp8 gemv ragged (default: all)
+usage: python scripts/gpu_check.py [section ...]
+  sections: gemm_bench gemm_sweep misc attn moe fp8 gemv ragged (default: all)
 gemm_bench also checks the outputs it times; the exit code is non-zero if one is wrong.
 """
 import math
@@ -87,6 +88,37 @@ def sec_gemm_bench():
             ref = ref * z.grad
         check(f"bench-correct {name}", out, ref, 0.05, 3e-2)
         del a, b, out, ref_out, ref, kw
+
+
+def sec_gemm_sweep():
+    """Per-tile cost model of the bf16 GEMM: M = 16384, N = 6144 (qkv fwd) with 128 x 256 tiles, K from 512 to 8192,
+    for each epilogue the training step uses.  The persistent kernel runs ceil(tiles / #SMs) rounds of one tile per
+    SM, so time / rounds = slope * K + intercept.  The slope is the mainloop's rate (printed as TFLOPS over all SMs);
+    the intercept is what every tile costs besides its K loop: pipeline fill, epilogue and stores.  Each epilogue runs
+    with the operand majors the step uses it with: dGELU in the dgrad layout (B stored [K, N]), the others forward."""
+    M, N = 16384, 6144
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    rounds = math.ceil(math.ceil(M / 128) * math.ceil(N / 256) / sms)
+    Ks = (512, 1024, 2048, 4096, 8192)
+    bias = torch.randn(N, device=dev, dtype=torch.bfloat16)
+    aux = torch.randn(M, N, device=dev, dtype=torch.bfloat16)
+    out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
+    epilogues = (("-", False, {}), ("bias", False, {"bias": bias}),
+                 ("bias+gelu+aux_out", False, {"bias": bias, "aux_out": aux, "act": 1}),
+                 ("dgelu", True, {"aux_in": aux, "act": 3}))
+    for name, tb, kw in epilogues:
+        per_round = []
+        for K in Ks:
+            a = torch.randn(M, K, device=dev, dtype=torch.bfloat16)
+            b = torch.randn((K, N) if tb else (N, K), device=dev, dtype=torch.bfloat16) * K ** -0.5
+            t = median_ms(lambda: _C.gemm(a, b, False, tb, out=out, block_n=256, **kw), flush=True)
+            per_round.append(t * 1e3 / rounds)
+            print(f"BENCH gemm_sweep {name:17s} M={M} N={N} K={K:5d}: {t:.3f} ms "
+                  f"{2 * M * N * K / t / 1e9:6.1f} TFLOPS  {per_round[-1]:.2f} us/round", flush=True)
+            del a, b
+        slope, icpt = np.polyfit(np.array(Ks, dtype=np.float64), np.array(per_round), 1)
+        print(f"FIT gemm_sweep {name:17s}: mainloop {2 * 128 * 256 * sms / slope / 1e6:.0f} TFLOPS, "
+              f"intercept {icpt:.1f} us/tile ({rounds} rounds of {sms} tiles)", flush=True)
 
 
 def sec_misc():
@@ -224,8 +256,8 @@ def sec_ragged():
         print(f"BENCH ragged_attention h{h} D{D} T{T}: {t * 1e3:.1f} us, {kv_bytes / t / 1e6:.0f} GB/s of K/V streamed")
 
 
-SECTIONS = {"gemm_bench": sec_gemm_bench, "misc": sec_misc, "attn": sec_attn, "moe": sec_moe, "fp8": sec_fp8,
-            "gemv": sec_gemv, "ragged": sec_ragged}
+SECTIONS = {"gemm_bench": sec_gemm_bench, "gemm_sweep": sec_gemm_sweep, "misc": sec_misc, "attn": sec_attn,
+            "moe": sec_moe, "fp8": sec_fp8, "gemv": sec_gemv, "ragged": sec_ragged}
 
 
 def card():
