@@ -7,7 +7,7 @@ The reference attends bidirectionally with an all-ones mask in its GPT benchmark
 (benchmark_one_case_gpt_bert.py:142-148); `causal=True` gives the usual decoder masking.
 
 H100 mapping: fused QKV projection (features ordered (head, {q,k,v}, D) so tensor-parallel splits are
-head splits), packed flash attention, GELU / bias / pre-activation fused into GEMM epilogues,
+head splits; with grouped-query attention (K/V head, {G query heads, k, v}, D)), packed flash attention, GELU / bias / pre-activation fused into GEMM epilogues,
 residual-add fused into LayerNorm, per-token fused cross-entropy.
 """
 from __future__ import annotations
@@ -29,6 +29,9 @@ class GPTConfig:
     hidden_size: int = 768
     num_hidden_layers: int = 12
     num_attention_heads: int = 12
+    # grouped-query attention: K/V heads shared by groups of num_attention_heads // num_key_value_heads query heads
+    # (None or num_attention_heads: multi-head attention)
+    num_key_value_heads: Optional[int] = None
     intermediate_size: Optional[int] = None
     max_position_embeddings: int = 1024
     layer_norm_eps: float = 1e-12
@@ -45,6 +48,20 @@ class GPTConfig:
         if self.intermediate_size is None:
             self.intermediate_size = 4 * self.hidden_size
         assert self.hidden_size % self.num_attention_heads == 0
+        kv = self.num_key_value_heads
+        assert kv is None or (kv > 0 and self.num_attention_heads % kv == 0), \
+            "num_key_value_heads must divide num_attention_heads"
+
+    @property
+    def grouped_query(self) -> bool:
+        return self.num_key_value_heads not in (None, self.num_attention_heads)
+
+    @property
+    def qkv_features(self) -> int:
+        """Output features of the fused QKV projection: 3 H, or (G + 2) Hkv D with grouped-query attention."""
+        if not self.grouped_query:
+            return 3 * self.hidden_size
+        return (self.num_attention_heads + 2 * self.num_key_value_heads) * (self.hidden_size // self.num_attention_heads)
 
 
 # (S, H, L, heads, V) of the reference's benchmark suite (benchmark/alpa/suite_manual_gpt.py:16-27)
@@ -75,8 +92,8 @@ class GPTBlock(nn.Module):
         kw = dict(device=device, dtype=cfg.dtype)
         std = cfg.initializer_range
         self.cfg = cfg
-        self.qkv_w = nn.Parameter(torch.randn(3 * H, H, **kw) * std)
-        self.qkv_b = nn.Parameter(torch.zeros(3 * H, **kw))
+        self.qkv_w = nn.Parameter(torch.randn(cfg.qkv_features, H, **kw) * std)
+        self.qkv_b = nn.Parameter(torch.zeros(cfg.qkv_features, **kw))
         self.proj_w = nn.Parameter(torch.randn(H, H, **kw) * std)
         self.proj_b = nn.Parameter(torch.zeros(H, **kw))
         self.ln1_g = nn.Parameter(torch.ones(H, **kw))
@@ -94,8 +111,14 @@ class GPTBlock(nn.Module):
         nh = cfg.num_attention_heads
         D = H // nh
         drop = dropout_seed is not None and getattr(cfg, "hidden_dropout_prob", 0.0) > 0.0
-        qkv = ops.linear(x, self.qkv_w, self.qkv_b).view(B, S, nh, 3, D)
-        o, _ = ops.attention_qkvpacked(qkv, 1.0 / math.sqrt(D), cfg.causal)
+        if cfg.grouped_query:
+            # features ordered (K/V head, {its G query heads, k, v}, D): a column split is a split over K/V heads
+            kvh = cfg.num_key_value_heads
+            qkv = ops.linear(x, self.qkv_w, self.qkv_b).view(B, S, kvh, nh // kvh + 2, D)
+            o, _ = ops.attention_gqa_packed(qkv, 1.0 / math.sqrt(D), cfg.causal)
+        else:
+            qkv = ops.linear(x, self.qkv_w, self.qkv_b).view(B, S, nh, 3, D)
+            o, _ = ops.attention_qkvpacked(qkv, 1.0 / math.sqrt(D), cfg.causal)
         a = ops.linear(o.view(B, S, H), self.proj_w, self.proj_b)
         if drop:
             a = ops.dropout_like(a, cfg.hidden_dropout_prob, dropout_seed, stream=2 * layer_idx + 1)
@@ -158,7 +181,8 @@ def gpt_lm_loss(logits: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
 
 def num_params(cfg: GPTConfig) -> int:
     H, I, V, L = cfg.hidden_size, cfg.intermediate_size, cfg.vocab_size, cfg.num_hidden_layers
-    per_layer = 3 * H * H + 3 * H + H * H + H + 2 * H + H * I + I + I * H + H + 2 * H
+    F = cfg.qkv_features
+    per_layer = F * H + F + H * H + H + 2 * H + H * I + I + I * H + H + 2 * H
     emb = V * H + cfg.max_position_embeddings * H + 2 * H
     dec = (0 if cfg.tie_word_embeddings else V * H) + V
     return L * per_layer + emb + dec

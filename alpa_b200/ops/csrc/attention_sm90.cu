@@ -17,6 +17,13 @@
 //   (S^T = K Q^T, dP^T = V dO^T, dV += P^T dO, dK += dS^T Q).  dQ: one warpgroup per 64 query rows with the forward's
 //   structure (S = Q K^T, dP = dO V^T, dQ += dS K).
 //
+// Grouped-query attention: query head hq = kv * group + g reads K/V head kv.  Forward and dQ CTAs take the K/V tiles of
+//   their query head's K/V head, and the G CTAs of one query tile of a group are adjacent in the grid, so they read the
+//   same K/V tiles at about the same time (from L2).  dK / dV: one warpgroup per (batch, K/V head, 64-key tile) streams
+//   the (Q, dO) tiles of every query head of the group through the ring and accumulates over all of them in registers.
+//   When those CTAs are too few to fill the GPU, the group is split into parts (ab_attention_bwd_splits) that write
+//   fp32 partials; attn_bwd_dkdv_reduce_kernel sums them in a fixed order.
+//
 // Masking (both directions): key j is visible to query i iff j < Skv and, when causal, j <= i + (Skv - Sq); Skv is the
 // device-side kv_len when one is given.  Head dims up to 128 in multiples of 8 run as 64 or 128 (TMA zero-fills).
 #include "kernels.h"
@@ -63,6 +70,13 @@ __device__ __forceinline__ void tma_tile(uint8_t* dst, const CUtensorMap* m, uin
 #pragma unroll
   for (int at = 0; at < DP / 64; ++at) tma_load_4d(dst + at * rows * 128, m, bar, at * 64, row0, h, b);
 }
+// The same from a [B, S, kv_heads, group, D] (query) tensor map.
+template <int DP>
+__device__ __forceinline__ void tma_tile_q(uint8_t* dst, const CUtensorMap* m, uint64_t* bar, int row0, int rows,
+                                           int g, int kv, int b) {
+#pragma unroll
+  for (int at = 0; at < DP / 64; ++at) tma_load_5d(dst + at * rows * 128, m, bar, at * 64, row0, g, kv, b);
+}
 
 __device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
   return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~static_cast<uintptr_t>(1023));
@@ -93,9 +107,11 @@ attn_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
   const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   const int wi = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t = lane & 3;
-  const int bh = blockIdx.y;
-  const int b = bh / a.heads, h = bh - b * a.heads;
-  const int q0 = blockIdx.x * kBQ;
+  const int G = a.group;
+  const int qt = blockIdx.x / G, gq = blockIdx.x - qt * G;  // x = query tile * G + head within the group
+  const int b = blockIdx.y / a.kv_heads, kvh = blockIdx.y - b * a.kv_heads;
+  const int hq = kvh * G + gq;
+  const int q0 = qt * kBQ;
   const int Skv = a.kv_len != nullptr ? min(a.Skv, *a.kv_len) : a.Skv;
   const int shift = Skv - a.Sq;  // causal: key j visible to query i iff j <= i + shift
   int kv_end = Skv;
@@ -105,14 +121,14 @@ attn_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
   auto issue_kv = [&](int j) {
     const int s = j & 1;
     mbar_expect_tx(&bar[1 + s], 2 * L::kKV);
-    tma_tile<DP>(sKV + 2 * s * L::kKV, &tk, &bar[1 + s], j * kTile, kTile, h, b);
-    tma_tile<DP>(sKV + (2 * s + 1) * L::kKV, &tv, &bar[1 + s], j * kTile, kTile, h, b);
+    tma_tile<DP>(sKV + 2 * s * L::kKV, &tk, &bar[1 + s], j * kTile, kTile, kvh, b);
+    tma_tile<DP>(sKV + (2 * s + 1) * L::kKV, &tv, &bar[1 + s], j * kTile, kTile, kvh, b);
   };
   if (threadIdx.x == 0) {
     for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1);
     mbar_fence_init();
     mbar_expect_tx(&bar[0], L::kQ);
-    tma_tile<DP>(sQ, &tq, &bar[0], q0, kBQ, h, b);
+    tma_tile_q<DP>(sQ, &tq, &bar[0], q0, kBQ, gq, kvh, b);
     for (int j = 0; j < 2 && j < n_tiles; ++j) issue_kv(j);
   }
   __syncthreads();
@@ -200,7 +216,7 @@ attn_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
     const int qi = qrow[r];
     const float inv = l > 0.f ? 1.f / l : 0.f;
     if (qi < a.Sq) {
-      __nv_bfloat16* og = a.o + (long long)b * a.o_stride_b + (long long)qi * a.o_stride_s + (long long)h * a.o_stride_h;
+      __nv_bfloat16* og = a.o + (long long)b * a.o_stride_b + (long long)qi * a.o_stride_s + (long long)hq * a.o_stride_h;
 #pragma unroll
       for (int dn = 0; dn < DP / 8; ++dn) {
         const int d = dn * 8 + 2 * t;
@@ -208,7 +224,7 @@ attn_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
           *reinterpret_cast<uint32_t*>(og + d) = pack_bf16x2(o[dn][2 * r] * inv, o[dn][2 * r + 1] * inv);
       }
       if (t == 0)
-        a.lse[((long long)b * a.heads + h) * a.Sq + qi] = l > 0.f ? (m_r[r] + __log2f(l)) * 0.69314718055994531f : -INFINITY;
+        a.lse[((long long)b * a.kv_heads * G + hq) * a.Sq + qi] = l > 0.f ? (m_r[r] + __log2f(l)) * 0.69314718055994531f : -INFINITY;
     }
   }
 }
@@ -222,7 +238,8 @@ struct AttnBwdSmem {
   static constexpr int kTotal = 6 * kT + 64 + 1024;   // two resident tiles + a two-stage ring of two tiles
 };
 
-// dK / dV of 64 keys: K, V resident, (Q, dO) tiles of 64 queries through the ring.
+// dK / dV of 64 keys: K, V resident, (Q, dO) tiles of 64 queries through the ring, for query heads [g0, g1) of the
+// group (part blockIdx.z of a.splits).  One part writes bf16; several write fp32 partials for the reduce kernel.
 template <int DP>
 __global__ void __launch_bounds__(128, 1)
 attn_bwd_dkdv_sm90_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
@@ -239,25 +256,28 @@ attn_bwd_dkdv_sm90_kernel(const __grid_constant__ CUtensorMap tq, const __grid_c
 
   const int wi = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
-  const int bh = blockIdx.y;
-  const int b = bh / f.heads, h = bh - b * f.heads;
+  const int G = f.group;
+  const int b = blockIdx.y / f.kv_heads, kvh = blockIdx.y - b * f.kv_heads;
+  const int g0 = blockIdx.z * G / a.splits, g1 = (blockIdx.z + 1) * G / a.splits;
   const int kv0 = blockIdx.x * kTile;
   const int Sq = f.Sq, Skv = f.Skv, shift = Skv - Sq;
   const int qt0 = (f.causal ? max(0, kv0 - shift) : 0) / kTile;
-  const int n_tiles = max(0, (Sq + kTile - 1) / kTile - qt0);
+  const int q_tiles = max(0, (Sq + kTile - 1) / kTile - qt0);  // per query head
+  const int n_tiles = (g1 - g0) * q_tiles;                       // step i: head g0 + i / q_tiles, tile i % q_tiles
 
   auto issue_q = [&](int i) {
     const int s = i & 1;
+    const int gh = g0 + i / q_tiles, q0 = (qt0 + i % q_tiles) * kTile;
     mbar_expect_tx(&bar[1 + s], 2 * L::kT);
-    tma_tile<DP>(sRing + 2 * s * L::kT, &tq, &bar[1 + s], (qt0 + i) * kTile, kTile, h, b);
-    tma_tile<DP>(sRing + (2 * s + 1) * L::kT, &tdo, &bar[1 + s], (qt0 + i) * kTile, kTile, h, b);
+    tma_tile_q<DP>(sRing + 2 * s * L::kT, &tq, &bar[1 + s], q0, kTile, gh, kvh, b);
+    tma_tile<DP>(sRing + (2 * s + 1) * L::kT, &tdo, &bar[1 + s], q0, kTile, kvh * G + gh, b);
   };
   if (threadIdx.x == 0) {
     for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1);
     mbar_fence_init();
     mbar_expect_tx(&bar[0], 2 * L::kT);
-    tma_tile<DP>(sK, &tk, &bar[0], kv0, kTile, h, b);
-    tma_tile<DP>(sV, &tv, &bar[0], kv0, kTile, h, b);
+    tma_tile<DP>(sK, &tk, &bar[0], kv0, kTile, kvh, b);
+    tma_tile<DP>(sV, &tv, &bar[0], kv0, kTile, kvh, b);
     for (int i = 0; i < 2 && i < n_tiles; ++i) issue_q(i);
   }
   __syncthreads();
@@ -268,14 +288,16 @@ attn_bwd_dkdv_sm90_kernel(const __grid_constant__ CUtensorMap tq, const __grid_c
 #pragma unroll
     for (int e = 0; e < 4; ++e) dk[i][e] = dv[i][e] = 0.f;
   const int key_row[2] = {kv0 + wi * 16 + g, kv0 + wi * 16 + g + 8};
-  const float* lse = f.lse + ((long long)b * f.heads + h) * Sq;
-  const float* delta = a.delta + ((long long)b * f.heads + h) * Sq;
   const uint32_t k_addr = smem_u32(sK), v_addr = smem_u32(sV);
   mbar_wait(&bar[0], 0);
 
   for (int i = 0; i < n_tiles; ++i) {
     const int s = i & 1;
-    const int q0 = (qt0 + i) * kTile;
+    const int gh = g0 + i / q_tiles;
+    const int q0 = (qt0 + i - (gh - g0) * q_tiles) * kTile;
+    const long long stat_row = ((long long)b * f.kv_heads * G + kvh * G + gh) * Sq;
+    const float* lse = f.lse + stat_row;
+    const float* delta = a.delta + stat_row;
     // per-query statistics of the 16 score columns this thread holds
     float lse2[8][2], dl[8][2];
 #pragma unroll
@@ -323,8 +345,21 @@ attn_bwd_dkdv_sm90_kernel(const __grid_constant__ CUtensorMap tq, const __grid_c
   for (int r = 0; r < 2; ++r) {
     const int key = key_row[r];
     if (key >= Skv) continue;
-    __nv_bfloat16* dkg = a.dk + (long long)b * a.dk_stride_b + (long long)key * a.dk_stride_s + (long long)h * a.dk_stride_h;
-    __nv_bfloat16* dvg = a.dv + (long long)b * a.dv_stride_b + (long long)key * a.dv_stride_s + (long long)h * a.dv_stride_h;
+    if (a.splits > 1) {
+      const long long dv_off = (long long)a.splits * f.B * f.kv_heads * Skv * f.D;  // dK partials, then dV partials
+      float* wk = a.ws + ((((long long)blockIdx.z * f.B + b) * f.kv_heads + kvh) * Skv + key) * f.D;
+#pragma unroll
+      for (int dn = 0; dn < DP / 8; ++dn) {
+        const int d = dn * 8 + 2 * t;
+        if (d < f.D) {
+          *reinterpret_cast<float2*>(wk + d) = make_float2(dk[dn][2 * r], dk[dn][2 * r + 1]);
+          *reinterpret_cast<float2*>(wk + dv_off + d) = make_float2(dv[dn][2 * r], dv[dn][2 * r + 1]);
+        }
+      }
+      continue;
+    }
+    __nv_bfloat16* dkg = a.dk + (long long)b * a.dk_stride_b + (long long)key * a.dk_stride_s + (long long)kvh * a.dk_stride_h;
+    __nv_bfloat16* dvg = a.dv + (long long)b * a.dv_stride_b + (long long)key * a.dv_stride_s + (long long)kvh * a.dv_stride_h;
 #pragma unroll
     for (int dn = 0; dn < DP / 8; ++dn) {
       const int d = dn * 8 + 2 * t;
@@ -334,6 +369,33 @@ attn_bwd_dkdv_sm90_kernel(const __grid_constant__ CUtensorMap tq, const __grid_c
       }
     }
   }
+}
+
+// dK / dV of a split group: the sum of the splits' fp32 partials in part order (fixed, so the result is the same from
+// run to run), dK scaled, rounded to bf16 once.  One thread per two adjacent head-dim elements.
+__global__ void attn_bwd_dkdv_reduce_kernel(const AttnBwdArgs a) {
+  const AttnArgs& f = a.f;
+  const int half_d = f.D / 2;
+  const long long n = (long long)f.B * f.kv_heads * f.Skv * half_d;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int d = (int)(i % half_d) * 2;
+  const long long row = i / half_d;  // (b, kv, key)
+  const int key = (int)(row % f.Skv);
+  const int kvh = (int)((row / f.Skv) % f.kv_heads);
+  const int b = (int)(row / ((long long)f.Skv * f.kv_heads));
+  const long long part = n * 2, dv_off = (long long)a.splits * part;
+  float2 sk = make_float2(0.f, 0.f), sv = make_float2(0.f, 0.f);
+  for (int p = 0; p < a.splits; ++p) {
+    const float2 x = *reinterpret_cast<const float2*>(a.ws + p * part + row * f.D + d);
+    const float2 y = *reinterpret_cast<const float2*>(a.ws + dv_off + p * part + row * f.D + d);
+    sk.x += x.x; sk.y += x.y;
+    sv.x += y.x; sv.y += y.y;
+  }
+  __nv_bfloat16* dkg = a.dk + (long long)b * a.dk_stride_b + (long long)key * a.dk_stride_s + (long long)kvh * a.dk_stride_h;
+  __nv_bfloat16* dvg = a.dv + (long long)b * a.dv_stride_b + (long long)key * a.dv_stride_s + (long long)kvh * a.dv_stride_h;
+  *reinterpret_cast<uint32_t*>(dkg + d) = pack_bf16x2(sk.x * f.scale, sk.y * f.scale);
+  *reinterpret_cast<uint32_t*>(dvg + d) = pack_bf16x2(sv.x, sv.y);
 }
 
 // dQ of 64 queries: Q, dO resident, (K, V) tiles through the ring.
@@ -353,9 +415,11 @@ attn_bwd_dq_sm90_kernel(const __grid_constant__ CUtensorMap tq, const __grid_con
 
   const int wi = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
-  const int bh = blockIdx.y;
-  const int b = bh / f.heads, h = bh - b * f.heads;
-  const int q0 = blockIdx.x * kTile;
+  const int G = f.group;
+  const int qt = blockIdx.x / G, gq = blockIdx.x - qt * G;  // x = query tile * G + head within the group
+  const int b = blockIdx.y / f.kv_heads, kvh = blockIdx.y - b * f.kv_heads;
+  const int hq = kvh * G + gq;
+  const int q0 = qt * kTile;
   const int Skv = f.Skv, shift = Skv - f.Sq;
   int kv_end = Skv;
   if (f.causal) kv_end = min(Skv, q0 + kTile + shift);
@@ -364,15 +428,15 @@ attn_bwd_dq_sm90_kernel(const __grid_constant__ CUtensorMap tq, const __grid_con
   auto issue_kv = [&](int j) {
     const int s = j & 1;
     mbar_expect_tx(&bar[1 + s], 2 * L::kT);
-    tma_tile<DP>(sRing + 2 * s * L::kT, &tk, &bar[1 + s], j * kTile, kTile, h, b);
-    tma_tile<DP>(sRing + (2 * s + 1) * L::kT, &tv, &bar[1 + s], j * kTile, kTile, h, b);
+    tma_tile<DP>(sRing + 2 * s * L::kT, &tk, &bar[1 + s], j * kTile, kTile, kvh, b);
+    tma_tile<DP>(sRing + (2 * s + 1) * L::kT, &tv, &bar[1 + s], j * kTile, kTile, kvh, b);
   };
   if (threadIdx.x == 0) {
     for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1);
     mbar_fence_init();
     mbar_expect_tx(&bar[0], 2 * L::kT);
-    tma_tile<DP>(sQ, &tq, &bar[0], q0, kTile, h, b);
-    tma_tile<DP>(sDO, &tdo, &bar[0], q0, kTile, h, b);
+    tma_tile_q<DP>(sQ, &tq, &bar[0], q0, kTile, gq, kvh, b);
+    tma_tile<DP>(sDO, &tdo, &bar[0], q0, kTile, hq, b);
     for (int j = 0; j < 2 && j < n_tiles; ++j) issue_kv(j);
   }
   __syncthreads();
@@ -383,7 +447,7 @@ attn_bwd_dq_sm90_kernel(const __grid_constant__ CUtensorMap tq, const __grid_con
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const bool ok = qrow[r] < f.Sq;
-    const long long idx = ((long long)b * f.heads + h) * f.Sq + qrow[r];
+    const long long idx = ((long long)b * f.kv_heads * G + hq) * f.Sq + qrow[r];
     lse2[r] = ok ? f.lse[idx] * 1.4426950408889634f : INFINITY;
     dlt[r] = ok ? a.delta[idx] : 0.f;
   }
@@ -427,7 +491,8 @@ attn_bwd_dq_sm90_kernel(const __grid_constant__ CUtensorMap tq, const __grid_con
   for (int r = 0; r < 2; ++r) {
     const int qi = qrow[r];
     if (qi >= f.Sq) continue;
-    __nv_bfloat16* dqg = a.dq + (long long)b * a.dq_stride_b + (long long)qi * a.dq_stride_s + (long long)h * a.dq_stride_h;
+    __nv_bfloat16* dqg = a.dq + (long long)b * a.dq_stride_b + (long long)qi * a.dq_stride_s + (long long)kvh * a.dq_stride_h +
+                         (long long)gq * a.dq_stride_g;
 #pragma unroll
     for (int dn = 0; dn < DP / 8; ++dn) {
       const int d = dn * 8 + 2 * t;
@@ -478,6 +543,15 @@ static int make_qkv_tmap(CUtensorMap* m, const __nv_bfloat16* p, int D, int S, i
   return make_tmap_bf16_4d(m, p, dims, strides, 64, rows);
 }
 
+// tensor map of the query view [B, S, kv_heads, group, D]; a group of one takes the K/V-head stride for its (only ever
+// zero) group coordinate, since a size-1 dim's stride can be anything
+static int make_q_tmap(CUtensorMap* m, const AttnArgs& a, int rows) {
+  const uint64_t dims[5] = {(uint64_t)a.D, (uint64_t)a.Sq, (uint64_t)a.group, (uint64_t)a.kv_heads, (uint64_t)a.B};
+  const uint64_t strides[4] = {(uint64_t)a.q_stride_s, (uint64_t)(a.group > 1 ? a.q_stride_g : a.q_stride_h),
+                               (uint64_t)a.q_stride_h, (uint64_t)a.q_stride_b};
+  return make_tmap_bf16_5d(m, a.q, dims, strides, 64, rows);
+}
+
 template <typename Kern>
 static bool set_smem(Kern k, int bytes) {
   return cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) == cudaSuccess;
@@ -486,9 +560,9 @@ static bool set_smem(Kern k, int bytes) {
 template <int DP, int WG>
 static int attn_fwd_launch(const AttnArgs& a, cudaStream_t st) {
   CUtensorMap tq, tk, tv;
-  if (make_qkv_tmap(&tq, a.q, a.D, a.Sq, a.heads, a.B, a.q_stride_s, a.q_stride_h, a.q_stride_b, 64 * WG)) return 10;
-  if (make_qkv_tmap(&tk, a.k, a.D, a.Skv, a.heads, a.B, a.k_stride_s, a.k_stride_h, a.k_stride_b, kTile)) return 11;
-  if (make_qkv_tmap(&tv, a.v, a.D, a.Skv, a.heads, a.B, a.v_stride_s, a.v_stride_h, a.v_stride_b, kTile)) return 12;
+  if (make_q_tmap(&tq, a, 64 * WG)) return 10;
+  if (make_qkv_tmap(&tk, a.k, a.D, a.Skv, a.kv_heads, a.B, a.k_stride_s, a.k_stride_h, a.k_stride_b, kTile)) return 11;
+  if (make_qkv_tmap(&tv, a.v, a.D, a.Skv, a.kv_heads, a.B, a.v_stride_s, a.v_stride_h, a.v_stride_b, kTile)) return 12;
   auto kern = attn_fwd_sm90_kernel<DP, WG>;
   constexpr int smem = AttnFwdSmem<DP, WG>::kTotal;
   static bool attr_set = false;
@@ -496,19 +570,35 @@ static int attn_fwd_launch(const AttnArgs& a, cudaStream_t st) {
     if (!set_smem(kern, smem)) return 20;
     attr_set = true;
   }
-  dim3 grid((a.Sq + 64 * WG - 1) / (64 * WG), a.B * a.heads);
+  dim3 grid((a.Sq + 64 * WG - 1) / (64 * WG) * a.group, a.B * a.kv_heads);
   kern<<<grid, WG * 128, smem, st>>>(tq, tk, tv, a, a.scale * 1.4426950408889634f);
   return cudaGetLastError() == cudaSuccess ? 0 : 30;
+}
+
+// Parts the dK / dV kernel splits each group of query heads into.  Its grid has B * kv_heads * ceil(Skv / 64) CTAs of
+// one warpgroup, and each holds about 97 KB of shared memory at head dim 128 (half at 64), so two or more share an SM.
+// When the grid is short of two CTAs per SM (grouped heads at tensor-parallel shapes: one K/V head per GPU), the group
+// is split into P parts, P the smallest divisor of the group size that gives at least 2 x SMs CTAs (else the whole
+// group, one head per CTA).  Equal parts keep the CTAs' work equal.  P > 1 costs one fp32 partial of dK and dV per part
+// and a reduce kernel; multi-head attention (group 1) never splits.
+static int bwd_splits(const AttnArgs& f) {
+  const long long ctas = (long long)f.B * f.kv_heads * ((f.Skv + kTile - 1) / kTile);
+  const long long want = 2LL * num_sms();
+  for (int p = 1; p < f.group; ++p)
+    if (f.group % p == 0 && ctas * p >= want) return p;
+  return f.group;
 }
 
 template <int DP>
 static int attn_bwd_launch(const AttnBwdArgs& a, cudaStream_t st) {
   const AttnArgs& f = a.f;
+  const int Hq = f.kv_heads * f.group;
   CUtensorMap tq, tk, tv, tdo;
-  if (make_qkv_tmap(&tq, f.q, f.D, f.Sq, f.heads, f.B, f.q_stride_s, f.q_stride_h, f.q_stride_b, kTile)) return 10;
-  if (make_qkv_tmap(&tk, f.k, f.D, f.Skv, f.heads, f.B, f.k_stride_s, f.k_stride_h, f.k_stride_b, kTile)) return 11;
-  if (make_qkv_tmap(&tv, f.v, f.D, f.Skv, f.heads, f.B, f.v_stride_s, f.v_stride_h, f.v_stride_b, kTile)) return 12;
-  if (make_qkv_tmap(&tdo, a.d_o, f.D, f.Sq, f.heads, f.B, f.o_stride_s, f.o_stride_h, f.o_stride_b, kTile)) return 13;
+  if (make_q_tmap(&tq, f, kTile)) return 10;
+  if (make_qkv_tmap(&tk, f.k, f.D, f.Skv, f.kv_heads, f.B, f.k_stride_s, f.k_stride_h, f.k_stride_b, kTile)) return 11;
+  if (make_qkv_tmap(&tv, f.v, f.D, f.Skv, f.kv_heads, f.B, f.v_stride_s, f.v_stride_h, f.v_stride_b, kTile)) return 12;
+  if (make_qkv_tmap(&tdo, a.d_o, f.D, f.Sq, Hq, f.B, f.o_stride_s, f.o_stride_h, f.o_stride_b, kTile)) return 13;
+  if (a.splits < 1 || a.splits > f.group || (a.splits > 1 && a.ws == nullptr)) return 14;
   auto kern = attn_bwd_dkdv_sm90_kernel<DP>;
   auto kern_dq = attn_bwd_dq_sm90_kernel<DP>;
   constexpr int smem = AttnBwdSmem<DP>::kTotal;
@@ -517,17 +607,22 @@ static int attn_bwd_launch(const AttnBwdArgs& a, cudaStream_t st) {
     if (!set_smem(kern, smem) || !set_smem(kern_dq, smem)) return 20;
     attr_set = true;
   }
-  const int rows = f.B * f.Sq * f.heads;
+  const int rows = f.B * f.Sq * Hq;
   if (f.D <= 64)
     attn_delta_kernel<8><<<(int)(((long long)rows * 8 + 255) / 256), 256, 0, st>>>(
-        a.d_o, f.o, a.delta, f.B, f.heads, f.Sq, f.D, f.o_stride_b, f.o_stride_s, f.o_stride_h);
+        a.d_o, f.o, a.delta, f.B, Hq, f.Sq, f.D, f.o_stride_b, f.o_stride_s, f.o_stride_h);
   else
     attn_delta_kernel<16><<<(int)(((long long)rows * 16 + 255) / 256), 256, 0, st>>>(
-        a.d_o, f.o, a.delta, f.B, f.heads, f.Sq, f.D, f.o_stride_b, f.o_stride_s, f.o_stride_h);
+        a.d_o, f.o, a.delta, f.B, Hq, f.Sq, f.D, f.o_stride_b, f.o_stride_s, f.o_stride_h);
   const float sl2 = f.scale * 1.4426950408889634f;
-  kern<<<dim3((f.Skv + kTile - 1) / kTile, f.B * f.heads), 128, smem, st>>>(tq, tk, tv, tdo, a, sl2);
+  kern<<<dim3((f.Skv + kTile - 1) / kTile, f.B * f.kv_heads, a.splits), 128, smem, st>>>(tq, tk, tv, tdo, a, sl2);
   if (cudaGetLastError() != cudaSuccess) return 30;
-  kern_dq<<<dim3((f.Sq + kTile - 1) / kTile, f.B * f.heads), 128, smem, st>>>(tq, tk, tv, tdo, a, sl2);
+  if (a.splits > 1) {
+    const long long n = (long long)f.B * f.kv_heads * f.Skv * (f.D / 2);
+    attn_bwd_dkdv_reduce_kernel<<<(int)((n + 255) / 256), 256, 0, st>>>(a);
+    if (cudaGetLastError() != cudaSuccess) return 32;
+  }
+  kern_dq<<<dim3((f.Sq + kTile - 1) / kTile * f.group, f.B * f.kv_heads), 128, smem, st>>>(tq, tk, tv, tdo, a, sl2);
   if (cudaGetLastError() != cudaSuccess) return 31;
   return 0;
 }
@@ -541,6 +636,8 @@ extern "C" int ab_attention_fwd(const ab::AttnArgs* a, int wide, cudaStream_t st
   if (a->D <= 64) return wide ? attn_fwd_launch<64, 2>(*a, st) : attn_fwd_launch<64, 1>(*a, st);
   return wide ? attn_fwd_launch<128, 2>(*a, st) : attn_fwd_launch<128, 1>(*a, st);
 }
+
+extern "C" int ab_attention_bwd_splits(const ab::AttnArgs* a) { return ab::bwd_splits(*a); }
 
 extern "C" int ab_attention_bwd(const ab::AttnBwdArgs* a, cudaStream_t st) {
   using namespace ab;

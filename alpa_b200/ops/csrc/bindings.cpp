@@ -269,18 +269,25 @@ void allreduce_oneshot(const Tensor& x, int64_t sym_local_ptr, int64_t mc_ptr, i
   g_launches += 1;
 }
 
+// q: [B,S,h,D] (multi-head) or [B,S,kv_heads,group,D] (grouped-query: query head kv * group + g uses K/V head kv);
+// k, v: [B,S,kv_heads,D].
 static void fill_attn_args(ab::AttnArgs& a, const Tensor& q, const Tensor& k, const Tensor& v,
                            double scale, bool causal) {
-  TORCH_CHECK(q.dim() == 4 && k.dim() == 4 && v.dim() == 4, "attention: [B,S,h,D] tensors");
+  TORCH_CHECK((q.dim() == 4 || q.dim() == 5) && k.dim() == 4 && v.dim() == 4,
+              "attention: q [B,S,h,D] or [B,S,kv_heads,group,D], k / v [B,S,kv_heads,D]");
   TORCH_CHECK(q.scalar_type() == at::kBFloat16 && k.scalar_type() == at::kBFloat16 &&
               v.scalar_type() == at::kBFloat16, "attention: bf16 only");
-  TORCH_CHECK(q.stride(3) == 1 && k.stride(3) == 1 && v.stride(3) == 1, "attention: D contiguous");
+  const bool grouped = q.dim() == 5;
+  TORCH_CHECK(q.stride(-1) == 1 && k.stride(3) == 1 && v.stride(3) == 1, "attention: D contiguous");
   a.q = bf16_ptr(q); a.k = bf16_ptr(k); a.v = bf16_ptr(v);
-  a.B = (int)q.size(0); a.Sq = (int)q.size(1); a.heads = (int)q.size(2); a.D = (int)q.size(3);
+  a.B = (int)q.size(0); a.Sq = (int)q.size(1); a.kv_heads = (int)q.size(2); a.D = (int)q.size(-1);
+  a.group = grouped ? (int)q.size(3) : 1;
+  TORCH_CHECK(a.group >= 1, "attention: empty query group");
   a.Skv = (int)k.size(1);
-  TORCH_CHECK(k.size(0) == a.B && v.size(0) == a.B && k.size(2) == a.heads && v.size(2) == a.heads &&
+  TORCH_CHECK(k.size(0) == a.B && v.size(0) == a.B && k.size(2) == a.kv_heads && v.size(2) == a.kv_heads &&
               k.size(3) == a.D && v.size(3) == a.D && v.size(1) == a.Skv, "attention: shape mismatch");
   a.q_stride_b = q.stride(0); a.q_stride_s = q.stride(1); a.q_stride_h = q.stride(2);
+  a.q_stride_g = grouped ? q.stride(3) : 0;
   a.k_stride_b = k.stride(0); a.k_stride_s = k.stride(1); a.k_stride_h = k.stride(2);
   a.v_stride_b = v.stride(0); a.v_stride_s = v.stride(1); a.v_stride_h = v.stride(2);
   a.scale = (float)scale;
@@ -298,11 +305,14 @@ std::vector<Tensor> attention_fwd(const Tensor& q, const Tensor& k, const Tensor
                 "attention: kv_len must be an int32 CUDA scalar");
     a.kv_len = kv_len->data_ptr<int>();
   }
-  Tensor o = torch::empty({a.B, a.Sq, a.heads, a.D}, q.options());
-  Tensor lse = torch::empty({a.B, a.heads, a.Sq}, q.options().dtype(at::kFloat));
+  const bool grouped = q.dim() == 5;
+  Tensor o = grouped ? torch::empty({a.B, a.Sq, a.kv_heads, a.group, a.D}, q.options())
+                     : torch::empty({a.B, a.Sq, a.kv_heads, a.D}, q.options());
+  Tensor lse = grouped ? torch::empty({a.B, a.kv_heads, a.group, a.Sq}, q.options().dtype(at::kFloat))
+                       : torch::empty({a.B, a.kv_heads, a.Sq}, q.options().dtype(at::kFloat));
   a.o = reinterpret_cast<__nv_bfloat16*>(o.data_ptr());
   a.lse = lse.data_ptr<float>();
-  a.o_stride_b = o.stride(0); a.o_stride_s = o.stride(1); a.o_stride_h = o.stride(2);
+  a.o_stride_b = o.stride(0); a.o_stride_s = o.stride(1); a.o_stride_h = a.D;  // contiguous: one stride per query head
   // 128-query tiles by default; ALPA_B200_ATTN_FWD=gen2 pins the 64-query-tile configuration (twice the CTAs).  The
   // kernel self-check (alpa_b200/ops/selfcheck.py) pins it when the default misbehaves on this GPU.
   static const bool narrow = [] {
@@ -382,7 +392,8 @@ Tensor dropout(const Tensor& x_in, double p, const Tensor& seed, int64_t stream,
 }
 
 // Backward of attention.  dq/dk/dv may be provided as (strided) views, e.g. slices of one packed
-// [B,S,h,3,D] buffer; otherwise contiguous [B,S,h,D] tensors are allocated.
+// [B,S,h,3,D] or [B,S,kv_heads,group+2,D] buffer; otherwise contiguous tensors shaped like q / k / v are allocated.
+// With a 5-D q, o and d_o are [B,S,kv_heads,group,D] and lse [B,kv_heads,group,Sq].
 std::vector<Tensor> attention_bwd(const Tensor& d_o_in, const Tensor& q, const Tensor& k, const Tensor& v,
                                   const Tensor& o_in, const Tensor& lse, double scale, bool causal,
                                   const OptTensor& dq_out, const OptTensor& dk_out, const OptTensor& dv_out) {
@@ -391,31 +402,49 @@ std::vector<Tensor> attention_bwd(const Tensor& d_o_in, const Tensor& q, const T
   Tensor o = o_in.contiguous();
   ab::AttnBwdArgs a;
   fill_attn_args(a.f, q, k, v, scale, causal);
-  TORCH_CHECK(lse.is_contiguous() && lse.scalar_type() == at::kFloat);
+  const int B = a.f.B, Hkv = a.f.kv_heads, G = a.f.group, Sq = a.f.Sq, Skv = a.f.Skv, D = a.f.D;
+  TORCH_CHECK(o.sizes() == q.sizes() && d_o.sizes() == q.sizes(), "attention_bwd: o / d_o must be shaped like q");
+  TORCH_CHECK(lse.is_contiguous() && lse.scalar_type() == at::kFloat && lse.numel() == (int64_t)B * Hkv * G * Sq,
+              "attention_bwd: lse must be contiguous fp32 [B, heads, Sq]");
   a.f.o = const_cast<__nv_bfloat16*>(bf16_ptr(o));
   a.f.lse = const_cast<float*>(lse.data_ptr<float>());
-  a.f.o_stride_b = o.stride(0); a.f.o_stride_s = o.stride(1); a.f.o_stride_h = o.stride(2);
+  a.f.o_stride_b = o.stride(0); a.f.o_stride_s = o.stride(1); a.f.o_stride_h = D;  // contiguous: per query head
   a.d_o = bf16_ptr(d_o);
-  const int B = a.f.B, H = a.f.heads, Sq = a.f.Sq, Skv = a.f.Skv, D = a.f.D;
-  Tensor delta = torch::empty({B, H, Sq}, q.options().dtype(at::kFloat));
-  auto pick = [&](const OptTensor& t, int S) {
+  Tensor delta = torch::empty({B, Hkv * G, Sq}, q.options().dtype(at::kFloat));
+  auto pick = [&](const OptTensor& t, const Tensor& like) {
     if (t.has_value() && t->defined()) {
-      TORCH_CHECK(t->dim() == 4 && t->stride(3) == 1 && t->scalar_type() == at::kBFloat16 && t->size(1) == S);
+      TORCH_CHECK(t->sizes() == like.sizes() && t->stride(-1) == 1 && t->scalar_type() == at::kBFloat16,
+                  "attention_bwd: gradient outputs must be bf16, shaped like q / k / v, D contiguous");
       return *t;
     }
-    return torch::empty({B, S, H, D}, q.options());
+    return torch::empty(like.sizes(), q.options());
   };
-  Tensor dq = pick(dq_out, Sq), dk = pick(dk_out, Skv), dv = pick(dv_out, Skv);
+  Tensor dq = pick(dq_out, q), dk = pick(dk_out, k), dv = pick(dv_out, v);
   a.delta = delta.data_ptr<float>();
   a.dq = reinterpret_cast<__nv_bfloat16*>(dq.data_ptr());
   a.dk = reinterpret_cast<__nv_bfloat16*>(dk.data_ptr());
   a.dv = reinterpret_cast<__nv_bfloat16*>(dv.data_ptr());
   a.dq_stride_b = dq.stride(0); a.dq_stride_s = dq.stride(1); a.dq_stride_h = dq.stride(2);
+  a.dq_stride_g = dq.dim() == 5 ? dq.stride(3) : 0;
   a.dk_stride_b = dk.stride(0); a.dk_stride_s = dk.stride(1); a.dk_stride_h = dk.stride(2);
   a.dv_stride_b = dv.stride(0); a.dv_stride_s = dv.stride(1); a.dv_stride_h = dv.stride(2);
+  a.splits = ab_attention_bwd_splits(&a.f);
+  Tensor ws;  // fp32 partials of a split group, from the caching allocator (capturable)
+  if (a.splits > 1) {
+    ws = torch::empty({2, a.splits, B, Hkv, Skv, D}, q.options().dtype(at::kFloat));
+    a.ws = ws.data_ptr<float>();
+  }
   AB_CHECK_RC(ab_attention_bwd(&a, cur_stream()), "ab_attention_bwd");
-  g_launches += 3;
+  g_launches += a.splits > 1 ? 4 : 3;
   return {dq, dk, dv};
+}
+
+// Parts the dK / dV kernel splits each query-head group into for these operands (1 = no split; see attention_sm90.cu).
+int64_t attention_bwd_splits(const Tensor& q, const Tensor& k, const Tensor& v) {
+  c10::cuda::CUDAGuard guard(q.device());
+  ab::AttnArgs a;
+  fill_attn_args(a, q, k, v, 1.0, false);
+  return ab_attention_bwd_splits(&a);
 }
 
 std::vector<Tensor> layernorm_fwd(const Tensor& x, const OptTensor& residual, const Tensor& gamma,
@@ -957,6 +986,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("attention_bwd", &attention_bwd, py::arg("d_o"), py::arg("q"), py::arg("k"), py::arg("v"), py::arg("o"),
         py::arg("lse"), py::arg("scale"), py::arg("causal"), py::arg("dq_out") = py::none(),
         py::arg("dk_out") = py::none(), py::arg("dv_out") = py::none());
+  m.def("attention_bwd_splits", &attention_bwd_splits, py::arg("q"), py::arg("k"), py::arg("v"));
   m.def("layernorm_fwd", &layernorm_fwd);
   m.def("layernorm_bwd", &layernorm_bwd);
   m.def("ce_stats", &ce_stats);

@@ -737,6 +737,20 @@ int make_tmap_bf16_4d(CUtensorMap* out, const void* ptr, const uint64_t* dims, c
   return r == CUDA_SUCCESS ? 0 : static_cast<int>(r);
 }
 
+int make_tmap_bf16_5d(CUtensorMap* out, const void* ptr, const uint64_t* dims, const uint64_t* strides_elems,
+                      uint32_t box_inner, uint32_t box_rows) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (!fn) return -1;
+  cuuint64_t d[5] = {dims[0], dims[1], dims[2], dims[3], dims[4]};
+  cuuint64_t st[4] = {strides_elems[0] * 2, strides_elems[1] * 2, strides_elems[2] * 2, strides_elems[3] * 2};
+  cuuint32_t bx[5] = {box_inner, box_rows, 1, 1, 1};
+  cuuint32_t es[5] = {1, 1, 1, 1, 1};
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(ptr), d, st, bx, es,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : static_cast<int>(r);
+}
+
 int make_tmap_bf16_3d(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t rows,
                       uint64_t batch, uint64_t row_stride_elems, uint64_t batch_stride_elems,
                       uint32_t box_inner, uint32_t box_rows) {

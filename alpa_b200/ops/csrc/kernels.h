@@ -52,17 +52,19 @@ struct AdamChunk {
   long long start;
 };
 
+// Grouped-query attention: query head hq = kv * group + g (g < group) attends with K/V head kv (HF's repeat_kv order);
+// group == 1 is multi-head attention.
 struct AttnArgs {
-  const __nv_bfloat16* q = nullptr;  // [B, S, heads, D] with arbitrary strides (elements)
-  const __nv_bfloat16* k = nullptr;
+  const __nv_bfloat16* q = nullptr;  // [B, S, kv_heads, group, D] with arbitrary strides (elements)
+  const __nv_bfloat16* k = nullptr;  // [B, S, kv_heads, D]
   const __nv_bfloat16* v = nullptr;
-  __nv_bfloat16* o = nullptr;
-  float* lse = nullptr;  // [B, heads, Sq] log-sum-exp (natural log) of scaled scores
-  int B = 0, heads = 0, Sq = 0, Skv = 0, D = 0;
-  long long q_stride_b = 0, q_stride_s = 0, q_stride_h = 0;
+  __nv_bfloat16* o = nullptr;        // [B, S, kv_heads * group, D]
+  float* lse = nullptr;  // [B, kv_heads * group, Sq] log-sum-exp (natural log) of scaled scores
+  int B = 0, kv_heads = 0, group = 1, Sq = 0, Skv = 0, D = 0;
+  long long q_stride_b = 0, q_stride_s = 0, q_stride_h = 0, q_stride_g = 0;  // q_stride_h: per K/V head
   long long k_stride_b = 0, k_stride_s = 0, k_stride_h = 0;
   long long v_stride_b = 0, v_stride_s = 0, v_stride_h = 0;
-  long long o_stride_b = 0, o_stride_s = 0, o_stride_h = 0;
+  long long o_stride_b = 0, o_stride_s = 0, o_stride_h = 0;                  // o_stride_h: per query head
   float scale = 1.f;
   int causal = 0;
   // optional device-side number of valid keys (<= Skv): lets one captured graph serve every decode position
@@ -87,16 +89,19 @@ struct GemvArgs {
 
 struct AttnBwdArgs {
   AttnArgs f;                          // q,k,v,o,lse + shapes/strides/scale/causal of the forward
-  const __nv_bfloat16* d_o = nullptr;  // [B,S,h,D], same strides as o
-  __nv_bfloat16* dk = nullptr;         // [B,Skv,heads,D] contiguous
+  const __nv_bfloat16* d_o = nullptr;  // [B,S,kv_heads*group,D], same strides as o
+  __nv_bfloat16* dk = nullptr;         // [B,Skv,kv_heads,D]
   __nv_bfloat16* dv = nullptr;
-  float* delta = nullptr;              // [B,heads,Sq] scratch: rowsum(dO * O)
-  // output strides in elements (b, s, h); D contiguous.  Lets dq/dk/dv be views of one packed
-  // [B,S,h,3,D] gradient buffer so the fused-QKV dgrad/wgrad GEMMs read it without a copy.
-  long long dq_stride_b = 0, dq_stride_s = 0, dq_stride_h = 0;
+  float* delta = nullptr;              // [B,kv_heads*group,Sq] scratch: rowsum(dO * O)
+  // output strides in elements (b, s, h[, g]); D contiguous.  Lets dq/dk/dv be views of one packed
+  // [B,S,h,3,D] (or [B,S,kv_heads,group+2,D]) gradient buffer so the fused-QKV dgrad/wgrad GEMMs read it without a copy.
+  long long dq_stride_b = 0, dq_stride_s = 0, dq_stride_h = 0, dq_stride_g = 0;
   long long dk_stride_b = 0, dk_stride_s = 0, dk_stride_h = 0;
   long long dv_stride_b = 0, dv_stride_s = 0, dv_stride_h = 0;
   __nv_bfloat16* dq = nullptr;
+  // group split of the dK / dV kernel (ab_attention_bwd_splits): splits > 1 needs ws, fp32 [2][splits][B][kv_heads][Skv][D]
+  int splits = 1;
+  float* ws = nullptr;
 };
 
 // Ragged 1-D token batch over a slot-addressed KV cache (serving with iteration-level batching).
@@ -174,6 +179,7 @@ struct PackArgs {
 extern "C" {
 int ab_attention_fwd(const ab::AttnArgs* a, int wide, cudaStream_t st);  // wide: 128-query tiles, else 64
 int ab_attention_bwd(const ab::AttnBwdArgs* a, cudaStream_t st);
+int ab_attention_bwd_splits(const ab::AttnArgs* a);  // parts the dK / dV kernel splits each query-head group into
 int ab_gemv_decode(const ab::GemvArgs* a, cudaStream_t st);
 int ab_ragged_attention(const ab::RaggedAttnArgs* a, cudaStream_t st);
 int ab_decode_attention(const ab::DecodeAttnArgs* a, cudaStream_t st);

@@ -17,6 +17,11 @@ int make_tmap_bf16_3d(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_
 int make_tmap_bf16_4d(CUtensorMap* out, const void* ptr, const uint64_t* dims, const uint64_t* strides_elems,
                       uint32_t box_inner, uint32_t box_rows);
 
+// 5-D form of the above, box (box_inner, box_rows, 1, 1, 1).  Used by the attention kernels on grouped query views
+// [B, S, kv_heads, group, D] whose two head strides are not one uniform stride (the packed GQA projection).
+int make_tmap_bf16_5d(CUtensorMap* out, const void* ptr, const uint64_t* dims, const uint64_t* strides_elems,
+                      uint32_t box_inner, uint32_t box_rows);
+
 int num_sms();
 
 }  // namespace ab

@@ -18,7 +18,7 @@ from alpa_b200.global_env import global_config
 __all__ = [
     "linear", "linear_act", "linear_dgrad", "linear_dgrad_add", "linear_wgrad", "bias_grad", "act_bwd", "layer_norm",
     "add_layer_norm", "layer_norm_bwd", "attention", "attention_bwd", "attention_qkvpacked",
-    "attention_qkvpacked_bwd", "embedding", "embedding_bwd",
+    "attention_qkvpacked_bwd", "attention_gqa_packed", "attention_gqa_packed_bwd", "embedding", "embedding_bwd",
     "cross_entropy", "cross_entropy_bwd", "fused_adamw_", "pipeline_marker", "uses_native",
     "bmm", "moe_dispatch", "moe_combine", "moe_combine_wgrad", "moe_top2_route", "linear_fp8", "linear_decode", "attention_decode", "decode_attention", "ragged_attention",
     "attention_cached", "attention_cached_", "quantize_mxfp8", "dequantize_mxfp8", "linear_mxfp8", "mx_pack_scale_atoms",
@@ -541,6 +541,90 @@ def _attn_packed_bwd(ctx, do, dlse):
 
 
 attention_qkvpacked.register_autograd(_attn_packed_bwd, setup_context=_attn_packed_setup)
+
+
+# ---- grouped-query packed variant: qkv is one [B, S, kv_heads, G + 2, D] tensor whose slots 0..G-1 are the query
+# heads kv * G + g of K/V head kv, slot G its K and slot G + 1 its V (HF's repeat_kv order).  A contiguous split of the
+# fused projection's output features is then a split over K/V heads that never splits a group.  G = 1 is the layout of
+# `attention_qkvpacked`.
+def _gqa_split(qkv):
+    G = qkv.shape[3] - 2
+    return qkv[:, :, :, :G], qkv[:, :, :, G], qkv[:, :, :, G + 1]
+
+
+def _gqa_native(qkv: Tensor, *others: Tensor) -> bool:
+    return (uses_native(qkv, *others) and qkv.shape[3] > 2 and qkv.shape[-1] % 8 == 0 and qkv.shape[-1] <= 128
+            and qkv.stride(-1) == 1)
+
+
+def _gqa_expand(q, k, v):
+    """q [B,Sq,Hkv,G,D], k / v [B,Skv,Hkv,D] -> [B,S,Hkv*G,D] each, K/V repeated per query head."""
+    B, Sq, Hkv, G, D = q.shape
+    rep = lambda t: t[:, :, :, None].expand(-1, -1, -1, G, -1).reshape(B, t.shape[1], Hkv * G, D)  # noqa: E731
+    return q.reshape(B, Sq, Hkv * G, D), rep(k), rep(v)
+
+
+def _gqa_attn_ref(q, k, v, scale, causal):
+    """PyTorch grouped-query attention: q [B,Sq,Hkv,G,D], k / v [B,Skv,Hkv,D] -> (o [B,Sq,Hkv,G,D], lse [B,Hkv,G,Sq]).
+    Rows that see no key give O = 0, as in `_attn_ref`."""
+    B, Sq, Hkv, G, D = q.shape
+    o, lse = _attn_ref(*_gqa_expand(q, k, v), scale, causal)
+    return o.view(B, Sq, Hkv, G, D), lse.view(B, Hkv, G, Sq)
+
+
+def _gqa_attn_ref_bwd(do, q, k, v, o, lse, scale, causal):
+    """Gradients of `_gqa_attn_ref`: dq like q, dk / dv like k / v (summed over each group in fp32)."""
+    B, Sq, Hkv, G, D = q.shape
+    Hq = Hkv * G
+    dq, dk, dv = attention_bwd(do.reshape(B, Sq, Hq, D), *_gqa_expand(q, k, v), o.reshape(B, Sq, Hq, D),
+                               lse.reshape(B, Hq, Sq), scale, causal)
+    group_sum = lambda t: t.view(B, -1, Hkv, G, D).float().sum(3).to(q.dtype)  # noqa: E731
+    return dq.view(B, Sq, Hkv, G, D), group_sum(dk), group_sum(dv)
+
+
+@torch.library.custom_op("alpa_b200::attention_gqa_packed", mutates_args=())
+def attention_gqa_packed(qkv: Tensor, scale: float, causal: bool) -> Tuple[Tensor, Tensor]:
+    """(o [B,S,Hkv,G,D], lse [B,Hkv,G,S]) = grouped-query softmax attention of qkv [B,S,Hkv,G+2,D]"""
+    q, k, v = _gqa_split(qkv)
+    if _gqa_native(qkv):
+        o, lse = _native().attention_fwd(q, k, v, scale, causal)
+        return o, lse
+    return _gqa_attn_ref(q, k, v, scale, causal)
+
+
+@attention_gqa_packed.register_fake
+def _(qkv, scale, causal):
+    B, S, Hkv, P, D = qkv.shape
+    return qkv.new_empty(B, S, Hkv, P - 2, D), qkv.new_empty(B, Hkv, P - 2, S, dtype=torch.float32)
+
+
+@torch.library.custom_op("alpa_b200::attention_gqa_packed_bwd", mutates_args=())
+def attention_gqa_packed_bwd(do: Tensor, qkv: Tensor, o: Tensor, lse: Tensor, scale: float, causal: bool) -> Tensor:
+    """dqkv [B,S,Hkv,G+2,D]: dQ in slots 0..G-1, dK (summed over the group) in slot G, dV in slot G + 1"""
+    q, k, v = _gqa_split(qkv)
+    G = q.shape[3]
+    dqkv = torch.empty(qkv.shape, device=qkv.device, dtype=qkv.dtype)
+    if _gqa_native(qkv, do, o):
+        _native().attention_bwd(do, q, k, v, o, lse, scale, causal, dqkv[:, :, :, :G], dqkv[:, :, :, G],
+                                dqkv[:, :, :, G + 1])
+        return dqkv
+    dqkv[:, :, :, :G], dqkv[:, :, :, G], dqkv[:, :, :, G + 1] = _gqa_attn_ref_bwd(do, q, k, v, o, lse, scale, causal)
+    return dqkv
+
+
+@attention_gqa_packed_bwd.register_fake
+def _(do, qkv, o, lse, scale, causal):
+    return torch.empty_like(qkv)
+
+
+def _attn_gqa_bwd(ctx, do, dlse):
+    if do is None:
+        return None, None, None
+    qkv, o, lse = ctx.saved_tensors
+    return attention_gqa_packed_bwd(do, qkv, o, lse, ctx.scale, ctx.causal), None, None
+
+
+attention_gqa_packed.register_autograd(_attn_gqa_bwd, setup_context=_attn_packed_setup)
 
 # =================================================================================================
 # embedding (token gather [+ position]) -- the reference lowers this to a one-hot matmul

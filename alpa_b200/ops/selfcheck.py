@@ -19,10 +19,19 @@ def _check_attention_fwd() -> str:
     C = ops.native_module()
     torch.manual_seed(0)
     worst = 0.0
-    for (B, H, S, D, causal) in [(2, 4, 256, 64, False), (1, 3, 384, 64, True), (4, 40, 1024, 64, False)]:
-        qkv = torch.randn(B, S, 3, H, D, device="cuda", dtype=torch.bfloat16)
-        q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
-        o, lse = C.attention_fwd(q, k, v, D ** -0.5, causal)                       # default dispatch
+    # (B, query heads, S, D, causal, group): group > 1 is a grouped-query call on a packed [B, S, H / G, G + 2, D] tensor
+    for (B, H, S, D, causal, G) in [(2, 4, 256, 64, False, 1), (1, 3, 384, 64, True, 1), (4, 40, 1024, 64, False, 1),
+                                    (2, 8, 320, 64, True, 4)]:
+        if G == 1:
+            qkv = torch.randn(B, S, 3, H, D, device="cuda", dtype=torch.bfloat16)
+            q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
+            o, lse = C.attention_fwd(q, k, v, D ** -0.5, causal)                   # default dispatch
+        else:
+            qkv = torch.randn(B, S, H // G, G + 2, D, device="cuda", dtype=torch.bfloat16)
+            q, k, v = qkv[:, :, :, :G], qkv[:, :, :, G], qkv[:, :, :, G + 1]
+            o, lse = C.attention_fwd(q, k, v, D ** -0.5, causal)
+            o, lse = o.reshape(B, S, H, D), lse.reshape(B, H, S)
+            q, k, v = q.reshape(B, S, H, D), k.repeat_interleave(G, 2), v.repeat_interleave(G, 2)
         qf, kf, vf = (t.float().permute(0, 2, 1, 3) for t in (q, k, v))
         s = torch.matmul(qf, kf.transpose(-1, -2)) * D ** -0.5
         if causal:
@@ -33,7 +42,7 @@ def _check_attention_fwd() -> str:
         err = (o.float() - ref).abs().max().item()
         err_l = (lse - ref_lse).abs().max().item()
         if not (err < 0.03 and err_l < 0.02):
-            return f"FAIL B{B} H{H} S{S} D{D} causal={causal}: max|o - ref| = {err:.4f}, max|lse - ref| = {err_l:.4f}"
+            return f"FAIL B{B} H{H} G{G} S{S} D{D} causal={causal}: max|o - ref| = {err:.4f}, max|lse - ref| = {err_l:.4f}"
         worst = max(worst, err)
     return f"ok (max abs err {worst:.4f})"
 

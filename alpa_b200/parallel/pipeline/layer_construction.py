@@ -118,7 +118,10 @@ def heavy_op_flops(func, args, kwargs, out) -> float:
             return 2.0 * _numel(o.shape) * _numel(w.shape[1:])
         if "alpa_b200.attention" in full and "bwd" not in full:
             q = args[0]
-            if q.dim() == 5:
+            if "gqa" in full:                      # [B, S, Hkv, G + 2, D]: G query heads per K/V head
+                B, S, Hkv, P, D = q.shape
+                H = Hkv * (P - 2)
+            elif q.dim() == 5:
                 B, S, H, _, D = q.shape
             else:
                 B, S, H, D = q.shape

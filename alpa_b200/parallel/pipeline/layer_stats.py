@@ -22,7 +22,8 @@ def _heavy_targets():
         _HEAVY = {a.mm.default, a.bmm.default, a.addmm.default, a.convolution.default, a.convolution_backward.default,
                   ab.linear.default, ab.linear_act.default, ab.linear_dgrad.default, ab.linear_dgrad_act.default, ab.linear_dgrad_add.default,
                   ab.linear_wgrad.default, ab.attention.default, ab.attention_bwd.default,
-                  ab.attention_qkvpacked.default, ab.attention_qkvpacked_bwd.default, ab.bmm.default}
+                  ab.attention_qkvpacked.default, ab.attention_qkvpacked_bwd.default,
+                  ab.attention_gqa_packed.default, ab.attention_gqa_packed_bwd.default, ab.bmm.default}
     return _HEAVY
 
 

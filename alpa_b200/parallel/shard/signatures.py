@@ -799,6 +799,34 @@ def rule_ab_attention_packed(node: fx.Node) -> OpSig:
     return sig
 
 
+def rule_ab_attention_gqa_packed(node: fx.Node) -> OpSig:
+    """attention_gqa_packed(qkv[B,S,Hkv,G+2,D]) / attention_gqa_packed_bwd(do, qkv, o, lse): batch and K/V heads
+    shard; the slots of one K/V head (its G query heads, K and V) stay together, so a group is never split."""
+    is_bwd = node.target == torch.ops.alpa_b200.attention_gqa_packed_bwd.default
+    qkv = node.args[1] if is_bwd else node.args[0]
+    sig = OpSig()
+    B, S_, Hkv, P, D = _shape(qkv)
+    G = P - 2
+    lb, lkv = sig.new(B), sig.new(Hkv)
+    ls, lslot, lg, ld = sig.new(S_, NOSHARD), sig.new(P, NOSHARD), sig.new(G, NOSHARD), sig.new(D, NOSHARD)
+    packed, act, stat = [lb, ls, lkv, lslot, ld], [lb, ls, lkv, lg, ld], [lb, lkv, lg, ls]
+    if is_bwd:
+        do, _, o, lse = node.args[:4]
+        sig.operands += [(do, act), (qkv, packed), (o, act), (lse, stat)]
+        t = _out_vals(node)[0]
+        sig.outputs.append((tuple(int(s) for s in t.shape), list(packed), t.dtype))
+        sig.follow = 1
+        sig.flops = 10.0 * B * Hkv * G * S_ * S_ * D
+    else:
+        sig.operands.append((qkv, packed))
+        vals = _val(node)
+        sig.outputs.append((tuple(int(s) for s in vals[0].shape), list(act), vals[0].dtype))
+        sig.outputs.append((tuple(int(s) for s in vals[1].shape), list(stat), vals[1].dtype))
+        sig.follow = 0
+        sig.flops = 4.0 * B * Hkv * G * S_ * S_ * D
+    return sig
+
+
 def _vocab_localize(arg_index: int, rows_arg: Optional[int] = None):
     def localize(node, ctx):
         args = list(node.args)
@@ -1145,6 +1173,7 @@ _reg([_ab.attention.default], rule_ab_attention)
 _reg([_ab.attention_bwd.default], rule_ab_attention_bwd)
 _reg([_ab.attention_cached.default], rule_ab_attention_cached)
 _reg([_ab.attention_qkvpacked.default, _ab.attention_qkvpacked_bwd.default], rule_ab_attention_packed)
+_reg([_ab.attention_gqa_packed.default, _ab.attention_gqa_packed_bwd.default], rule_ab_attention_gqa_packed)
 _reg([_ab.embedding.default], rule_ab_embedding)
 _reg([_ab.embedding_bwd.default], rule_ab_embedding_bwd)
 _reg([_ab.cross_entropy.default], rule_ab_cross_entropy)

@@ -2,7 +2,7 @@
 calls after 5 warm-ups).  The kernels' numerics are checked by the GPU tests under tests/.
 
 usage: python scripts/gpu_check.py [section ...]
-  sections: gemm_bench gemm_sweep misc attn moe fp8 gemv ragged (default: all)
+  sections: gemm_bench gemm_sweep misc attn attn_gqa moe fp8 gemv ragged (default: all)
 gemm_bench also checks the outputs it times; the exit code is non-zero if one is wrong.
 """
 import math
@@ -157,6 +157,44 @@ def sec_attn():
         print(f"BENCH attn bwd B{B} H{H} S{S} D{D} causal={int(causal)}: {t:.3f} ms {2.5 * fl / t / 1e9:.1f} TFLOPS", flush=True)
 
 
+def sec_attn_gqa():
+    """Grouped-query attention against what a user does without it: the multi-head kernel on K/V expanded with
+    repeat_interleave (the expansion itself not timed), whose backward needs the group sum of dK / dV on top, and
+    torch's SDPA with enable_gqa.  Shapes: Llama-3-8B-like on one GPU; one GPU of an 8-way tensor-parallel 70B-like
+    model (one K/V head: the dK / dV group split); multi-query attention."""
+    for (B, S, Hq, Hkv, D, causal) in [(4, 2048, 32, 8, 128, True), (1, 4096, 8, 1, 128, True),
+                                       (8, 1024, 32, 1, 64, False)]:
+        G = Hq // Hkv
+        qkv = torch.randn(B, S, Hkv, G + 2, D, device=dev, dtype=torch.bfloat16)
+        q, k, v = qkv[:, :, :, :G], qkv[:, :, :, G], qkv[:, :, :, G + 1]
+        scale = 1.0 / math.sqrt(D)
+        fl = 4 * B * Hq * S * S * D * (0.5 if causal else 1.0)
+        tag = f"B{B} S{S} Hq{Hq} Hkv{Hkv} D{D} causal={int(causal)}"
+        splits = _C.attention_bwd_splits(q, k, v)
+
+        def row(name, t, flops):
+            print(f"BENCH attn_gqa {tag} {name}: {t:.3f} ms {flops / t / 1e9:.1f} TFLOPS", flush=True)
+
+        row("gqa fwd", median_ms(lambda: _C.attention_fwd(q, k, v, scale, causal), flush=True), fl)
+        o, lse = _C.attention_fwd(q, k, v, scale, causal)
+        do = torch.randn_like(o)
+        row(f"gqa bwd (dK/dV group split {splits})",
+            median_ms(lambda: _C.attention_bwd(do, q, k, v, o, lse, scale, causal), flush=True), 2.5 * fl)
+        qe = q.reshape(B, S, Hq, D)
+        ke, ve = (x.repeat_interleave(G, dim=2) for x in (k, v))
+        row("mha fwd on expanded K/V", median_ms(lambda: _C.attention_fwd(qe, ke, ve, scale, causal), flush=True), fl)
+        oe, lsee = _C.attention_fwd(qe, ke, ve, scale, causal)
+        doe = do.reshape(B, S, Hq, D)
+
+        def mha_bwd():
+            dq, dk, dv = _C.attention_bwd(doe, qe, ke, ve, oe, lsee, scale, causal)
+            return dk.view(B, S, Hkv, G, D).sum(3), dv.view(B, S, Hkv, G, D).sum(3)
+        row("mha bwd on expanded K/V + group sum", median_ms(mha_bwd, flush=True), 2.5 * fl)
+        qt, kt, vt = qe.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)
+        row("sdpa(lib) enable_gqa fwd", median_ms(lambda: torch.nn.functional.scaled_dot_product_attention(
+            qt, kt, vt, is_causal=causal, scale=scale, enable_gqa=True), flush=True), fl)
+
+
 def sec_moe():
     """MoE routing, dispatch, combine and expert GEMM at the MoE-2.4B layer shapes (E = 16, M = 1024, H = 4096)."""
     G, S, E, M, H = 4, 2048, 16, 1024, 4096
@@ -257,7 +295,7 @@ def sec_ragged():
 
 
 SECTIONS = {"gemm_bench": sec_gemm_bench, "gemm_sweep": sec_gemm_sweep, "misc": sec_misc, "attn": sec_attn,
-            "moe": sec_moe, "fp8": sec_fp8, "gemv": sec_gemv, "ragged": sec_ragged}
+            "attn_gqa": sec_attn_gqa, "moe": sec_moe, "fp8": sec_fp8, "gemv": sec_gemv, "ragged": sec_ragged}
 
 
 def card():
