@@ -25,6 +25,8 @@ inline const __nv_bfloat16* bf16_ptr(const OptTensor& t) {
   return reinterpret_cast<const __nv_bfloat16*>(t->data_ptr());
 }
 
+inline bool aligned(const void* p, uintptr_t bytes) { return reinterpret_cast<uintptr_t>(p) % bytes == 0; }
+
 // Number of alpa_b200 CUDA kernels launched by this process (bench.py reports it as gpu_launches).
 static std::atomic<long long> g_launches{0};
 #define AB_CHECK_RC(rc, what) TORCH_CHECK((rc) == 0, what, " failed with code ", (rc))
@@ -333,6 +335,8 @@ Tensor ragged_attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_
   TORCH_CHECK(k_cache.stride(2) == 1 && k_cache.stride(1) == k_cache.size(2) && v_cache.strides() == k_cache.strides() &&
               v_cache.sizes() == k_cache.sizes(), "ragged_attention: cache rows must be dense");
   TORCH_CHECK(k_cache.size(1) == q.size(1) && k_cache.size(2) == q.size(2));
+  TORCH_CHECK(aligned(k_cache.data_ptr(), 16) && aligned(v_cache.data_ptr(), 16),
+              "ragged_attention: cache bases must be 16-byte aligned (16-byte K loads)");
   TORCH_CHECK(seq_start.scalar_type() == at::kInt && ctx_len.scalar_type() == at::kInt && seq_start.is_contiguous() &&
               ctx_len.is_contiguous() && seq_start.numel() == q.size(0) && ctx_len.numel() == q.size(0) &&
               seq_start.is_cuda() && ctx_len.is_cuda(), "ragged_attention: seq_start / ctx_len must be int32 CUDA [T]");
@@ -539,13 +543,21 @@ void ce_grad_(Tensor logits, const Tensor& labels, const Tensor& gstats, const T
 Tensor embedding_fwd(const Tensor& ids, const OptTensor& pos, const Tensor& wte, const OptTensor& wpe,
                      int64_t vocab_start) {
   TORCH_CHECK(ids.scalar_type() == at::kLong && ids.is_contiguous() && wte.is_contiguous());
+  TORCH_CHECK(wte.dim() == 2 && wte.scalar_type() == at::kBFloat16 && aligned(wte.data_ptr(), 16),
+              "embedding_fwd: wte must be a 16-byte aligned bf16 [V, H] table");
+  const bool has_pos = pos.has_value() && pos->defined();
+  TORCH_CHECK(has_pos == (wpe.has_value() && wpe->defined()), "embedding_fwd: pos and wpe must be given together");
+  if (has_pos)
+    TORCH_CHECK(wpe->scalar_type() == at::kBFloat16 && wpe->is_contiguous() && wpe->dim() == 2 &&
+                wpe->size(1) == wte.size(1) && aligned(wpe->data_ptr(), 16),
+                "embedding_fwd: wpe must be a contiguous, 16-byte aligned bf16 [P, H] table");
   c10::cuda::CUDAGuard guard(wte.device());
   const int T = (int)ids.numel(), H = (int)wte.size(1);
   auto shape = ids.sizes().vec();
   shape.push_back(H);
   Tensor out = torch::empty(shape, wte.options());
   const int64_t* pp = nullptr;
-  if (pos.has_value() && pos->defined()) {
+  if (has_pos) {
     TORCH_CHECK(pos->scalar_type() == at::kLong && pos->is_contiguous() && pos->numel() == T);
     pp = pos->data_ptr<int64_t>();
   }
@@ -597,6 +609,19 @@ std::vector<Tensor> adam_build_tables(const std::vector<Tensor>& grads, const st
                 vs[i].is_contiguous());
     TORCH_CHECK(masters[i].scalar_type() == at::kFloat && ms[i].scalar_type() == at::kFloat &&
                 vs[i].scalar_type() == at::kFloat);
+    const int64_t n_i = masters[i].numel();
+    const bool has_param = params[i].has_value() && params[i]->defined();
+    TORCH_CHECK(grads[i].numel() == n_i && ms[i].numel() == n_i && vs[i].numel() == n_i &&
+                (!has_param || params[i]->numel() == n_i),
+                "adam_build_tables: grad, master, m, v and param ", i, " must have the same number of elements");
+    TORCH_CHECK(aligned(masters[i].data_ptr(), 16) && aligned(ms[i].data_ptr(), 16) && aligned(vs[i].data_ptr(), 16),
+                "adam_build_tables: master, m and v ", i, " must be 16-byte aligned (float4 accesses)");
+    TORCH_CHECK(grads[i].scalar_type() != at::kBFloat16 || aligned(grads[i].data_ptr(), 8),
+                "adam_build_tables: bf16 grad ", i, " must be 8-byte aligned");
+    TORCH_CHECK(grads[i].scalar_type() != at::kFloat || aligned(grads[i].data_ptr(), 16),
+                "adam_build_tables: fp32 grad ", i, " must be 16-byte aligned");
+    TORCH_CHECK(!has_param || (params[i]->is_contiguous() && aligned(params[i]->data_ptr(), 8)),
+                "adam_build_tables: bf16 param ", i, " must be contiguous and 8-byte aligned");
     tt[i].grad = grads[i].data_ptr();
     tt[i].grad_is_bf16 = grads[i].scalar_type() == at::kBFloat16;
     TORCH_CHECK(tt[i].grad_is_bf16 || grads[i].scalar_type() == at::kFloat);
@@ -665,6 +690,21 @@ static ab::MoePeers moe_peers(const Tensor& local, const std::vector<int64_t>& p
   return p;
 }
 
+// expert / slot int64 and weight bf16, all [G, S, K] with G, S taken from `tok` ([G, S, M] activations); the rows
+// of `tok` and of the expert buffer `buf` are accessed 16 bytes at a time.
+static void check_moe_args(const char* what, const Tensor& tok, const Tensor& buf, const Tensor& expert,
+                           const Tensor& slot, const OptTensor& weight) {
+  TORCH_CHECK(tok.dim() == 3 && buf.dim() == 3 && tok.size(2) == buf.size(2), what,
+              ": activations must be [G, S, M] and the expert buffer [E, G*C, M]");
+  TORCH_CHECK(expert.scalar_type() == at::kLong && slot.scalar_type() == at::kLong, what, ": expert and slot must be int64");
+  TORCH_CHECK(expert.dim() == 3 && expert.size(0) == tok.size(0) && expert.size(1) == tok.size(1) &&
+              slot.sizes() == expert.sizes(), what, ": expert and slot must be [G, S, K] matching the activations");
+  if (weight.has_value() && weight->defined())
+    TORCH_CHECK(weight->sizes() == expert.sizes() && weight->is_contiguous(), what, ": weight must be contiguous [G, S, K]");
+  TORCH_CHECK(aligned(tok.data_ptr(), 16) && aligned(buf.data_ptr(), 16), what,
+              ": activations and expert buffer must be 16-byte aligned");
+}
+
 std::vector<Tensor> moe_top2_route(const Tensor& gates, int64_t capacity) {
   TORCH_CHECK(gates.is_cuda() && gates.scalar_type() == at::kFloat && gates.is_contiguous() && gates.dim() == 3);
   c10::cuda::CUDAGuard guard(gates.device());
@@ -683,6 +723,7 @@ void moe_dispatch_(const Tensor& x, const Tensor& expert, const Tensor& slot, co
                    int64_t capacity, std::vector<int64_t> peer_ptrs, int64_t g_off) {
   TORCH_CHECK(x.is_contiguous() && expert.is_contiguous() && slot.is_contiguous() && d.is_contiguous());
   TORCH_CHECK(x.scalar_type() == at::kBFloat16 && d.scalar_type() == at::kBFloat16 && expert.scalar_type() == at::kLong);
+  check_moe_args("moe_dispatch", x, d, expert, slot, weight);
   c10::cuda::CUDAGuard guard(x.device());
   const int G = (int)x.size(0), S = (int)x.size(1), M = (int)x.size(2), K = (int)expert.size(2);
   const int G_total = (int)(d.size(1) / capacity);
@@ -697,13 +738,15 @@ Tensor moe_combine(const Tensor& eo, const Tensor& expert, const Tensor& slot, c
                    std::vector<int64_t> peer_ptrs, int64_t g_off) {
   TORCH_CHECK(eo.is_contiguous() && expert.is_contiguous() && slot.is_contiguous());
   TORCH_CHECK(eo.scalar_type() == at::kBFloat16 && expert.scalar_type() == at::kLong);
+  TORCH_CHECK(expert.dim() == 3 && eo.dim() == 3, "moe_combine: expert must be [G, S, K] and eo [E, G*C, M]");
+  Tensor out = torch::empty({expert.size(0), expert.size(1), eo.size(2)}, eo.options());
+  check_moe_args("moe_combine", out, eo, expert, slot, weight);
   c10::cuda::CUDAGuard guard(eo.device());
   const int G = (int)expert.size(0), S = (int)expert.size(1), K = (int)expert.size(2), M = (int)eo.size(2);
   const int64_t peers = peer_ptrs.empty() ? 1 : (int64_t)peer_ptrs.size();
   const int G_total = peer_ptrs.empty() ? G : G * (int)peers;
   const int C = (int)(eo.size(1) / G_total);
   ab::MoePeers p = moe_peers(eo, peer_ptrs, eo.size(0) * peers);
-  Tensor out = torch::empty({G, S, M}, eo.options());
   AB_CHECK_RC(ab_moe_combine(&p, expert.data_ptr<int64_t>(), slot.data_ptr<int64_t>(), bf16_ptr(weight),
                              reinterpret_cast<__nv_bfloat16*>(out.data_ptr()), G, S, K, M, C, (int)g_off, G_total,
                              cur_stream()), "ab_moe_combine");
@@ -715,6 +758,7 @@ Tensor moe_combine_wgrad(const Tensor& dout, const Tensor& eo, const Tensor& exp
                          std::vector<int64_t> peer_ptrs, int64_t g_off) {
   TORCH_CHECK(eo.is_contiguous() && expert.is_contiguous() && slot.is_contiguous() && dout.is_contiguous());
   TORCH_CHECK(eo.scalar_type() == at::kBFloat16 && dout.scalar_type() == at::kBFloat16);
+  check_moe_args("moe_combine_wgrad", dout, eo, expert, slot, OptTensor());
   c10::cuda::CUDAGuard guard(eo.device());
   const int G = (int)expert.size(0), S = (int)expert.size(1), K = (int)expert.size(2), M = (int)eo.size(2);
   const int64_t peers = peer_ptrs.empty() ? 1 : (int64_t)peer_ptrs.size();
@@ -923,6 +967,9 @@ Tensor decode_attention(const Tensor& q, const Tensor& k_new, const Tensor& v_ne
               k_cache.stride(2) == k_cache.size(3), "decode_attention: caches must be bf16 [B, S_max, heads, D], rows dense");
   TORCH_CHECK(kv_len.is_cuda() && kv_len.scalar_type() == at::kInt && kv_len.numel() == 1,
               "decode_attention: kv_len must be an int32 CUDA scalar");
+  TORCH_CHECK(aligned(q.data_ptr(), 16) && aligned(k_new.data_ptr(), 16) && aligned(v_new.data_ptr(), 16) &&
+              aligned(k_cache.data_ptr(), 16) && aligned(v_cache.data_ptr(), 16),
+              "decode_attention: q, k_new, v_new and the caches must start on 16-byte boundaries (16-byte accesses)");
   c10::cuda::CUDAGuard guard(q.device());
   ab::DecodeAttnArgs a;
   a.q = bf16_ptr(q); a.k_new = bf16_ptr(k_new); a.v_new = bf16_ptr(v_new);

@@ -41,21 +41,24 @@ moe_top2_route_kernel(const float* __restrict__ gates, int64_t* __restrict__ exp
   // ---- top-2 experts of every token
   for (int s = tid; s < S; s += kRouteThreads) {
     const float* row = gg + (size_t)s * E;
-    float b1 = -INFINITY, b2 = -INFINITY;
-    int i1 = 0, i2 = 0;
+    float b1 = -INFINITY;
+    int i1 = 0;
     for (int e = 0; e < E; ++e) {
       const float v = row[e];
       if (v > b1) {
-        b2 = b1; i2 = i1;
         b1 = v; i1 = e;
-      } else if (v > b2) {
+      }
+    }
+    // second choice: argmax of the gates with the first choice's gate replaced by 0 (first index of the maximum).
+    // fp32 softmax underflows to exact zeros, so this can pick i1 again, as the dense top2_gating does.
+    float b2 = -INFINITY;
+    int i2 = 0;
+    for (int e = 0; e < E; ++e) {
+      const float v = e == i1 ? 0.f : row[e];
+      if (v > b2) {
         b2 = v; i2 = e;
       }
     }
-    if (E == 1) i2 = 0;
-    else if (b2 == -INFINITY || (i2 == i1)) i2 = (i1 == 0) ? 1 : 0;
-    // the oracle masks the first choice to 0 and takes argmax again: if every other gate is <= 0 it picks
-    // the first index (which may be i1's neighbour); gates are softmax outputs (> 0) so this cannot happen
     ex[2 * s] = i1;
     ex[2 * s + 1] = i2;
   }

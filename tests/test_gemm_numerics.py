@@ -35,7 +35,8 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from test_kernel_numerics import EPS32, TOL32, Checker, bf16_rule, fp32_rule  # noqa: E402
+from test_kernel_numerics import (EPS32, TOL32, Checker, attn_fwd_ref, bf16_rule, fp32_rule, ln_fwd_ref,  # noqa: E402
+                                  visible)
 
 F64 = torch.float64
 BF16 = torch.bfloat16
@@ -845,8 +846,33 @@ def test_primitives_dispatch():
         dz = P.linear_dgrad_act(dyh, w1, zh, act)
         ref, base, _, _, _ = epilogue_ref(dyh.to(F64).reshape(T, F4) @ w1f, act=did, aux_in=zh.reshape(T, H))
         ck.bf16(f"linear_dgrad_act {act}", f"linear_dgrad_act {act}", dz.reshape(T, H), ref, base)
-    r = torch.randn(4, T // 4, H, generator=g, device="cuda").to(BF16)
+    # linear with bias, linear_dgrad, linear_wgrad
+    y = P.linear(x, w1, b1)
+    ref, base, _, _, _ = epilogue_ref(xf @ w1f.t(), bias=b1)
+    ck.bf16("linear", "linear bias", y.reshape(T, F4), ref, base)
     dyh = torch.randn(4, T // 4, F4, generator=g, device="cuda").to(BF16)
+    dx = P.linear_dgrad(dyh, w1)
+    ref = dyh.to(F64).reshape(T, F4) @ w1f
+    ck.bf16("linear_dgrad", "linear_dgrad", dx.reshape(T, H), ref, _bf(ref))
+    dw = P.linear_wgrad(dyh, x)
+    ref = dyh.to(F64).reshape(T, F4).t() @ xf
+    ck.bf16("linear_wgrad", "linear_wgrad", dw, ref, _bf(ref))
+    # layer_norm (output only; mean / rstd are checked with the kernel in tests/test_kernel_numerics.py)
+    gam = (1 + 0.1 * torch.randn(H, generator=g, device="cuda")).to(BF16)
+    bet = (0.1 * torch.randn(H, generator=g, device="cuda")).to(BF16)
+    yn, _, _ = P.layer_norm(x, gam, bet, 1e-5)
+    ref = ln_fwd_ref(x.reshape(T, H), gam, bet, 1e-5)[0]
+    ck.bf16("layer_norm", "layer_norm", yn.reshape(T, H), ref, _bf(ref))
+    # attention_qkvpacked (causal and full), baseline rounds the unnormalised P as the kernel does
+    qkv = torch.randn(2, 256, 4, 3, 64, generator=g, device="cuda").to(BF16)
+    for causal in (False, True):
+        o, _ = P.attention_qkvpacked(qkv, 0.125, causal)
+        q_, k_, v_ = (qkv[:, :, :, i] for i in range(3))
+        vis = visible(256, 256, causal, device="cuda")
+        ref, _ = attn_fwd_ref(q_, k_, v_, 0.125, vis)
+        base, _ = attn_fwd_ref(q_, k_, v_, 0.125, vis, p_round=_bf)
+        ck.bf16("attention_qkvpacked", f"attention_qkvpacked causal={causal}", o, ref, base)
+    r = torch.randn(4, T // 4, H, generator=g, device="cuda").to(BF16)
     dx = P.linear_dgrad_add(dyh, w1, r)
     ref, base, _, _, _ = epilogue_ref(dyh.to(F64).reshape(T, F4) @ w1f, residual=r.reshape(T, H))
     ck.bf16("linear_dgrad_add", "linear_dgrad_add", dx.reshape(T, H), ref, base)

@@ -1,55 +1,8 @@
 """GPU checks of the iteration-level batching path (new this round; runs after the other GPU tests)."""
-import os
-import sys
-
 import pytest
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from test_gpu_kernels import check  # noqa: E402
-
 pytestmark = pytest.mark.gpu
-
-
-def test_ragged_attention_numerics():
-    """Ragged 1-D attention over a slot-addressed KV cache (OPT-2.7B/TP1 head shapes), with and without ALiBi, against
-    the fp32 PyTorch path of the same op."""
-    from alpa_b200 import ops
-    from alpa_b200.ops import primitives as P
-    torch.manual_seed(0)
-    dev = "cuda"
-    fails = []
-    for (h, D, lens, new) in [(4, 64, [37, 1, 300, 129], [5, 1, 1, 129]), (32, 80, [512, 77, 2048, 1000], [1, 1, 1, 64]),
-                              (8, 128, [16, 4000], [16, 1])]:
-        slots = sum(lens) + 64
-        kc = torch.randn(slots + 1, h, D, device=dev, dtype=torch.bfloat16)
-        vc = torch.randn(slots + 1, h, D, device=dev, dtype=torch.bfloat16)
-        starts, s = [], 7
-        for n in lens:
-            starts.append(s)
-            s += n + 3
-        seq_start, ctx_len = [], []
-        for st, n, k in zip(starts, lens, new):            # the last `k` tokens of each sequence are queries
-            for j in range(n - k, n):
-                seq_start.append(st)
-                ctx_len.append(j + 1)
-        seq_start += [0, 0]
-        ctx_len += [0, 0]                                   # padding tokens
-        T = len(seq_start)
-        q = torch.randn(T, h, 3, D, device=dev, dtype=torch.bfloat16)[:, :, 0]          # strided view like qkv
-        ss = torch.tensor(seq_start, dtype=torch.int32, device=dev)
-        cl = torch.tensor(ctx_len, dtype=torch.int32, device=dev)
-        mc = max(lens)
-        for alibi in (None, torch.linspace(0.01, 0.2, h, device=dev)):
-            got = ops.ragged_attention(q, kc, vc, ss, cl, D ** -0.5, mc, alibi)
-            old = P.global_config.use_native_kernels
-            P.global_config.use_native_kernels = False
-            try:
-                ref = ops.ragged_attention(q.float(), kc.float(), vc.float(), ss, cl, D ** -0.5, mc, alibi)
-            finally:
-                P.global_config.use_native_kernels = old
-            check(fails, f"ragged_attention h{h} D{D} T{T} alibi={alibi is not None}", got, ref, 2e-2, 2e-2)
-    assert not fails, "\n".join(fails)
 
 
 def test_forward_1d_on_gpu_matches_padded_forward():
