@@ -26,9 +26,6 @@ class GlobalConfig:
         # Compute dtype policy of the kernel library: bf16 tensors run the sm_90a kernels,
         # everything else (CPU, fp32) runs the PyTorch reference implementation of the same op.
         self.use_native_kernels = True
-        # If True the ops refuse to fall back to PyTorch on a CUDA device (used by bench/tests to
-        # guarantee the native path is the one measured).
-        self.require_native_kernels = _env_flag("ALPA_B200_REQUIRE_NATIVE", False)
         # Capture each compiled SPMD program in a CUDA graph after warm-up.
         self.use_cuda_graph = _env_flag("ALPA_B200_CUDA_GRAPH", False)
         # Use NVLink peer-memory fused compute+collective kernels where the plan allows.

@@ -8,8 +8,10 @@ Every primitive is a ``torch.library`` custom op in the ``alpa_b200`` namespace 
 * an autograd formula expressed in other primitives (so fwd+bwd trace to one flat graph), and
 * a sharding signature used by the auto-sharding planner (``alpa_b200/parallel/shard``).
 
-`native_available()` tells whether the compiled extension could be loaded.  On a CUDA device the ops
-fail loudly when it is missing unless ALPA_B200_ALLOW_FALLBACK=1.
+Every op decides between its kernel and its reference through one gate, ``primitives._kernels``: CPU tensors,
+``global_config.use_native_kernels = False`` and dtypes the kernel does not serve take the reference silently; on a
+CUDA device a missing extension (`native_available()` is False) is an error unless ALPA_B200_ALLOW_FALLBACK=1; a
+layout the kernel cannot take runs the reference and is recorded in ``primitives.library_fallbacks()``.
 """
 import importlib
 import os

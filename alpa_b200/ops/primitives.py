@@ -7,6 +7,7 @@ hand-written sm_90a kernels, and the *same* op names appear in traced graphs, pl
 from __future__ import annotations
 
 import math
+from functools import cache
 from typing import List, Optional, Tuple
 
 import torch
@@ -19,8 +20,8 @@ __all__ = [
     "linear", "linear_act", "linear_dgrad", "linear_dgrad_add", "linear_wgrad", "bias_grad", "act_bwd", "layer_norm",
     "add_layer_norm", "layer_norm_bwd", "attention", "attention_bwd", "attention_gqa_packed",
     "attention_gqa_packed_bwd", "embedding", "embedding_bwd",
-    "cross_entropy", "cross_entropy_bwd", "fused_adamw_", "pipeline_marker", "uses_native",
-    "bmm", "moe_dispatch", "moe_combine", "moe_combine_wgrad", "moe_top2_route", "linear_fp8", "linear_decode", "attention_decode", "decode_attention", "ragged_attention",
+    "cross_entropy", "cross_entropy_bwd", "fused_adamw_", "pipeline_marker",
+    "bmm", "moe_dispatch", "moe_combine", "moe_combine_wgrad", "moe_top2_route", "linear_fp8", "linear_decode", "decode_attention", "ragged_attention",
     "attention_cached", "attention_cached_", "quantize_mxfp8", "dequantize_mxfp8", "linear_mxfp8", "mx_pack_scale_atoms",
     "mx_unpack_scale_atoms", "pack_tiles", "unpack_tiles", "packed_nbytes",
     "dropout", "dropout_like", "dropout_keep_mask",
@@ -30,57 +31,56 @@ _ACT_IDS = {"none": 0, "gelu": 1, "relu": 2}
 _DACT_IDS = {"gelu": 3, "relu": 4}
 
 
-def _native():
-    from alpa_b200 import ops
-    return ops.native_module()
-
-
-def uses_native(*tensors: Tensor) -> bool:
-    """True if the sm_90a kernels serve this call: CUDA + bf16 activations.  On CUDA/bf16 a missing
-    extension is an error (no silent eager fallback) unless ALPA_B200_ALLOW_FALLBACK=1."""
-    ts = [t for t in tensors if t is not None]
-    if not ts or not all(t.is_cuda for t in ts):
-        return False
-    if not global_config.use_native_kernels:
-        return False
-    if not all(t.dtype == torch.bfloat16 for t in ts if t.is_floating_point()):
-        return False
-    from alpa_b200 import ops
-    if ops.native_available():
-        return True
-    if ops.allow_fallback():
-        return False
-    raise RuntimeError("alpa_b200: CUDA bf16 tensors but the sm_90a extension is not built/loaded "
-                       "(run `python -m alpa_b200.ops.build`; set ALPA_B200_ALLOW_FALLBACK=1 to use PyTorch)")
-
-
 _FALLBACK_SEEN = set()
 
 
+def _kernels(op: str, *tensors: Optional[Tensor], dtypes=(torch.bfloat16,), unsupported=None):
+    """The sm_90a extension if its kernel serves this call of `op`, else None (the caller runs its PyTorch reference).
+
+    Expected reference paths return None silently: a tensor off CUDA, `global_config.use_native_kernels` off, or a
+    floating tensor whose dtype is not in `dtypes` (None: any dtype).  A missing extension is an error unless
+    ALPA_B200_ALLOW_FALLBACK=1.  `unsupported` is the caller's reason why the kernel cannot take this layout, or a
+    function returning it (called only past the checks above, so the reference path builds no kernel operand views);
+    such a call is a library fallback: it is recorded for `library_fallbacks()`, warned about once, and returns None."""
+    ts = [t for t in tensors if t is not None]
+    if not ts or not global_config.use_native_kernels or not all(t.is_cuda for t in ts):
+        return None
+    if dtypes is not None and not all(t.dtype in dtypes for t in ts if t.is_floating_point()):
+        return None
+    from alpa_b200 import ops
+    if not ops.native_available():
+        if ops.allow_fallback():
+            return None
+        raise RuntimeError(f"alpa_b200: {op} on CUDA but the sm_90a extension is not built/loaded "
+                           "(run `python -m alpa_b200.ops.build`; set ALPA_B200_ALLOW_FALLBACK=1 to use PyTorch)")
+    if callable(unsupported):
+        unsupported = unsupported()
+    if unsupported is not None:
+        key = (op, unsupported, tuple((tuple(t.shape), tuple(t.stride())) for t in ts))
+        if key not in _FALLBACK_SEEN:
+            _FALLBACK_SEEN.add(key)
+            import logging
+            logging.getLogger(__name__).warning(
+                "alpa_b200: %s falls back to PyTorch (%s; operand shapes / strides %s)", *key)
+        return None
+    return ops.native_module()
+
+
 def library_fallbacks():
-    """Operand layouts for which a primitive fell back to a PyTorch library kernel although the sm_90a extension is
-    loaded (shape / stride / alignment outside the wgmma kernel's TMA constraints).  One warning per distinct
-    layout is logged; tests and benchmarks can assert this stays empty."""
+    """(op, reason, operand shapes / strides) of every call that ran a PyTorch reference on CUDA although the sm_90a
+    extension is loaded, because the kernel cannot take the operands' layout.  One warning per distinct entry is
+    logged; tests and benchmarks can assert this stays empty."""
     return sorted(_FALLBACK_SEEN)
 
 
-def _gemm_ok(*mats: Tensor) -> bool:
+def _gemm_unsupported(*mats: Tensor) -> Optional[str]:
+    """Why the wgmma GEMM's TMA descriptors cannot describe these operands, or None."""
     for m in mats:
-        bad = None
         if m.dim() not in (2, 3) or m.stride(-1) != 1 or m.shape[-1] % 8 or m.shape[-2] % 8:
-            bad = "shape"
-        elif m.stride(-2) % 8 or m.data_ptr() % 16:
-            bad = "alignment"
-        if bad is not None:
-            key = (bad, tuple(m.shape), tuple(m.stride()))
-            if key not in _FALLBACK_SEEN:
-                _FALLBACK_SEEN.add(key)
-                import logging
-                logging.getLogger(__name__).warning(
-                    "alpa_b200: GEMM operand %s (strides %s) is outside the sm_90a kernel's TMA constraints (%s): "
-                    "this call uses the PyTorch library kernel", tuple(m.shape), tuple(m.stride()), bad)
-            return False
-    return True
+            return "GEMM operand shape"
+        if m.stride(-2) % 8 or m.data_ptr() % 16:
+            return "GEMM operand alignment"
+    return None
 
 
 def _as2d(x: Tensor) -> Tensor:
@@ -104,11 +104,9 @@ def _act_fn(z: Tensor, act: str) -> Tensor:
 @torch.library.custom_op("alpa_b200::linear", mutates_args=())
 def linear(x: Tensor, w: Tensor, b: Optional[Tensor] = None) -> Tensor:
     """y[..., N] = x[..., K] @ w[N, K]^T + b[N]"""
-    if uses_native(x, w, b):
-        x2 = _as2d(x)
-        if _gemm_ok(x2, w):
-            y = _native().gemm(x2, w, False, False, bias=b)
-            return y.view(*x.shape[:-1], w.shape[0])
+    x2 = cache(lambda: _as2d(x))
+    if C := _kernels("linear", x, w, b, unsupported=lambda: _gemm_unsupported(x2(), w)):
+        return C.gemm(x2(), w, False, False, bias=b).view(*x.shape[:-1], w.shape[0])
     return F.linear(x, w, b)
 
 
@@ -120,13 +118,12 @@ def _(x, w, b=None):
 @torch.library.custom_op("alpa_b200::linear_act", mutates_args=())
 def linear_act(x: Tensor, w: Tensor, b: Optional[Tensor], act: str) -> Tuple[Tensor, Tensor]:
     """(act(z), z) with z = x @ w^T + b; the pre-activation z is kept for the backward pass."""
-    if uses_native(x, w, b):
-        x2 = _as2d(x)
-        if _gemm_ok(x2, w):
-            z = torch.empty(x2.shape[0], w.shape[0], device=x.device, dtype=x.dtype)
-            y = _native().gemm(x2, w, False, False, bias=b, aux_out=z, act=_ACT_IDS[act])
-            shp = (*x.shape[:-1], w.shape[0])
-            return y.view(shp), z.view(shp)
+    x2 = cache(lambda: _as2d(x))
+    if C := _kernels("linear_act", x, w, b, unsupported=lambda: _gemm_unsupported(x2(), w)):
+        z = torch.empty(x2().shape[0], w.shape[0], device=x.device, dtype=x.dtype)
+        y = C.gemm(x2(), w, False, False, bias=b, aux_out=z, act=_ACT_IDS[act])
+        shp = (*x.shape[:-1], w.shape[0])
+        return y.view(shp), z.view(shp)
     z = F.linear(x, w, b)
     return _act_fn(z, act), z
 
@@ -140,11 +137,9 @@ def _(x, w, b, act):
 @torch.library.custom_op("alpa_b200::linear_dgrad", mutates_args=())
 def linear_dgrad(dy: Tensor, w: Tensor) -> Tensor:
     """dx[..., K] = dy[..., N] @ w[N, K]"""
-    if uses_native(dy, w):
-        d2 = _as2d(dy)
-        if _gemm_ok(d2, w):
-            dx = _native().gemm(d2, w, False, True)
-            return dx.view(*dy.shape[:-1], w.shape[1])
+    d2 = cache(lambda: _as2d(dy))
+    if C := _kernels("linear_dgrad", dy, w, unsupported=lambda: _gemm_unsupported(d2(), w)):
+        return C.gemm(d2(), w, False, True).view(*dy.shape[:-1], w.shape[1])
     return torch.matmul(dy, w)
 
 
@@ -156,11 +151,11 @@ def _(dy, w):
 @torch.library.custom_op("alpa_b200::linear_dgrad_act", mutates_args=())
 def linear_dgrad_act(dy: Tensor, w: Tensor, z: Tensor, act: str) -> Tensor:
     """dz = (dy @ w) * act'(z): the activation backward fused into the dgrad epilogue."""
-    if uses_native(dy, w, z):
-        d2, z2 = _as2d(dy), _as2d(z)
-        if _gemm_ok(d2, w) and z2.is_contiguous():
-            dx = _native().gemm(d2, w, False, True, aux_in=z2, act=_DACT_IDS[act])
-            return dx.view(*dy.shape[:-1], w.shape[1])
+    v = cache(lambda: (_as2d(dy), _as2d(z)))
+    if C := _kernels("linear_dgrad_act", dy, w, z, unsupported=lambda: _gemm_unsupported(v()[0], w) or (
+                     None if v()[1].is_contiguous() else "pre-activation not contiguous")):
+        d2, z2 = v()
+        return C.gemm(d2, w, False, True, aux_in=z2, act=_DACT_IDS[act]).view(*dy.shape[:-1], w.shape[1])
     return _act_bwd_ref(torch.matmul(dy, w), z, act)
 
 
@@ -176,11 +171,12 @@ def linear_dgrad_add(dy: Tensor, w: Tensor, r: Optional[Tensor]) -> Tensor:
     tensor-parallel group that must not add it again (dx is a partial sum there)."""
     if r is None:
         return linear_dgrad._init_fn(dy, w)
-    if uses_native(dy, w, r):
-        d2, r2 = _as2d(dy), _as2d(r)
-        if _gemm_ok(d2, w) and r2.is_contiguous() and r2.shape == (d2.shape[0], w.shape[1]):
-            dx = _native().gemm(d2, w, False, True, residual=r2)
-            return dx.view(*dy.shape[:-1], w.shape[1])
+    v = cache(lambda: (_as2d(dy), _as2d(r)))
+    if C := _kernels("linear_dgrad_add", dy, w, r, unsupported=lambda: _gemm_unsupported(v()[0], w) or (
+                     None if v()[1].is_contiguous() and v()[1].shape == (v()[0].shape[0], w.shape[1])
+                     else "addend not a contiguous [M, K]")):
+        d2, r2 = v()
+        return C.gemm(d2, w, False, True, residual=r2).view(*dy.shape[:-1], w.shape[1])
     return torch.matmul(dy, w) + r
 
 
@@ -192,10 +188,9 @@ def _(dy, w, r):
 @torch.library.custom_op("alpa_b200::linear_wgrad", mutates_args=())
 def linear_wgrad(dy: Tensor, x: Tensor) -> Tensor:
     """dw[N, K] = dy[..., N]^T @ x[..., K]"""
-    if uses_native(dy, x):
-        d2, x2 = _as2d(dy), _as2d(x)
-        if _gemm_ok(d2, x2):
-            return _native().gemm(d2, x2, True, True)
+    v = cache(lambda: (_as2d(dy), _as2d(x)))
+    if C := _kernels("linear_wgrad", dy, x, unsupported=lambda: _gemm_unsupported(*v())):
+        return C.gemm(*v(), True, True)
     d2 = dy.reshape(-1, dy.shape[-1])
     x2 = x.reshape(-1, x.shape[-1])
     return torch.matmul(d2.t(), x2)
@@ -209,12 +204,12 @@ def _(dy, x):
 @torch.library.custom_op("alpa_b200::bias_grad", mutates_args=())
 def bias_grad(dy: Tensor) -> Tensor:
     """db[N] = sum over all leading dims of dy[..., N]"""
-    if uses_native(dy):
-        d2 = _as2d(dy)
-        if d2.shape[1] % 8 == 0 and d2.stride(0) % 8 == 0 and d2.data_ptr() % 16 == 0:
-            out = torch.zeros(d2.shape[1], device=dy.device, dtype=torch.float32)
-            _native().colsum_(d2, out)
-            return out.to(dy.dtype)
+    d2 = cache(lambda: _as2d(dy))
+    if C := _kernels("bias_grad", dy, unsupported=lambda: None if d2().shape[1] % 8 == 0 and d2().stride(0) % 8 == 0
+                     and d2().data_ptr() % 16 == 0 else "rows not 16-byte aligned"):
+        out = torch.zeros(dy.shape[-1], device=dy.device, dtype=torch.float32)
+        C.colsum_(d2(), out)
+        return out.to(dy.dtype)
     return dy.reshape(-1, dy.shape[-1]).sum(0)
 
 
@@ -304,11 +299,16 @@ def _ln_ref(x: Tensor, g: Tensor, b: Tensor, eps: float):
     return y.to(x.dtype), mean, rstd
 
 
+def _ln_unsupported(H: int) -> Optional[str]:
+    """Why the LayerNorm kernels (8-element vectors, at most 8192 elements per row) cannot take rows of H, or None."""
+    return None if H % 8 == 0 and H <= 8192 else "row length not a multiple of 8 up to 8192"
+
+
 @torch.library.custom_op("alpa_b200::layer_norm", mutates_args=())
 def layer_norm(x: Tensor, g: Tensor, b: Tensor, eps: float) -> Tuple[Tensor, Tensor, Tensor]:
     """(y, mean, rstd); statistics are fp32 with shape x.shape[:-1]."""
-    if uses_native(x, g, b) and x.shape[-1] % 8 == 0 and x.shape[-1] <= 8192:
-        y, mean, rstd, _ = _native().layernorm_fwd(x.contiguous(), None, g, b, eps, False)
+    if C := _kernels("layer_norm", x, g, b, unsupported=_ln_unsupported(x.shape[-1])):
+        y, mean, rstd, _ = C.layernorm_fwd(x.contiguous(), None, g, b, eps, False)
         return y, mean.view(x.shape[:-1]), rstd.view(x.shape[:-1])
     return _ln_ref(x, g, b, eps)
 
@@ -322,8 +322,8 @@ def _(x, g, b, eps):
 @torch.library.custom_op("alpa_b200::add_layer_norm", mutates_args=())
 def add_layer_norm(x: Tensor, r: Tensor, g: Tensor, b: Tensor, eps: float) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
     """s = x + r; (layer_norm(s), s, mean, rstd) in one pass."""
-    if uses_native(x, r, g, b) and x.shape[-1] % 8 == 0 and x.shape[-1] <= 8192:
-        y, mean, rstd, s = _native().layernorm_fwd(x.contiguous(), r.contiguous(), g, b, eps, True)
+    if C := _kernels("add_layer_norm", x, r, g, b, unsupported=_ln_unsupported(x.shape[-1])):
+        y, mean, rstd, s = C.layernorm_fwd(x.contiguous(), r.contiguous(), g, b, eps, True)
         return y, s, mean.view(x.shape[:-1]), rstd.view(x.shape[:-1])
     s = x + r
     y, mean, rstd = _ln_ref(s, g, b, eps)
@@ -341,12 +341,11 @@ def layer_norm_bwd(dy: Tensor, x: Tensor, g: Tensor, mean: Tensor, rstd: Tensor,
                    dres: Optional[Tensor]) -> Tuple[Tensor, Tensor, Tensor]:
     """(dx [+ dres], dgamma, dbeta) of y = layer_norm(x)."""
     H = x.shape[-1]
-    if uses_native(dy, x, g) and H % 8 == 0 and H <= 8192:
+    if C := _kernels("layer_norm_bwd", dy, x, g, unsupported=_ln_unsupported(H)):
         dg = torch.zeros(H, device=x.device, dtype=torch.float32)
         db = torch.zeros(H, device=x.device, dtype=torch.float32)
-        dx = _native().layernorm_bwd(dy.contiguous(), x.contiguous(), g, mean.reshape(-1).contiguous(),
-                                     rstd.reshape(-1).contiguous(),
-                                     dres.contiguous() if dres is not None else None, dg, db)
+        dx = C.layernorm_bwd(dy.contiguous(), x.contiguous(), g, mean.reshape(-1).contiguous(),
+                             rstd.reshape(-1).contiguous(), dres.contiguous() if dres is not None else None, dg, db)
         return dx, dg.to(g.dtype), db.to(g.dtype)
     xf, df = x.float(), dy.float()
     xh = (xf - mean[..., None]) * rstd[..., None]
@@ -424,11 +423,19 @@ def _finite_lse(lse):
     return lse.masked_fill(lse == float("-inf"), 0.0)
 
 
+def _attn_unsupported(D: int, stride: int = 1) -> Optional[str]:
+    """Why the sm_90a attention kernels cannot take head dim D at element stride `stride` (they need a contiguous
+    multiple of 8 up to 128), or None."""
+    if D % 8 or D > 128:
+        return "head dim not a multiple of 8 up to 128"
+    return None if stride == 1 else "head dim not contiguous"
+
+
 @torch.library.custom_op("alpa_b200::attention", mutates_args=())
 def attention(q: Tensor, k: Tensor, v: Tensor, scale: float, causal: bool) -> Tuple[Tensor, Tensor]:
     """(o [B,S,h,D], lse [B,h,S]) = softmax(q k^T * scale [+ causal mask]) v"""
-    if uses_native(q, k, v) and q.shape[-1] % 8 == 0 and q.shape[-1] <= 128 and q.stride(-1) == 1:
-        o, lse = _native().attention_fwd(q, k, v, scale, causal)
+    if C := _kernels("attention", q, k, v, unsupported=_attn_unsupported(q.shape[-1], q.stride(-1))):
+        o, lse = C.attention_fwd(q, k, v, scale, causal)
         return o, lse
     return _attn_ref(q, k, v, scale, causal)
 
@@ -442,9 +449,19 @@ def _(q, k, v, scale, causal):
 @torch.library.custom_op("alpa_b200::attention_bwd", mutates_args=())
 def attention_bwd(do: Tensor, q: Tensor, k: Tensor, v: Tensor, o: Tensor, lse: Tensor, scale: float,
                   causal: bool) -> Tuple[Tensor, Tensor, Tensor]:
-    if uses_native(do, q, k, v, o) and q.shape[-1] % 8 == 0 and q.shape[-1] <= 128 and q.stride(-1) == 1:
-        dq, dk, dv = _native().attention_bwd(do, q, k, v, o, lse, scale, causal)
+    if C := _kernels("attention_bwd", do, q, k, v, o, unsupported=_attn_unsupported(q.shape[-1], q.stride(-1))):
+        dq, dk, dv = C.attention_bwd(do, q, k, v, o, lse, scale, causal)
         return dq, dk, dv
+    return _attn_ref_bwd(do, q, k, v, o, lse, scale, causal)
+
+
+@attention_bwd.register_fake
+def _(do, q, k, v, o, lse, scale, causal):
+    return (q.new_empty(q.shape), k.new_empty(k.shape), v.new_empty(v.shape))
+
+
+def _attn_ref_bwd(do, q, k, v, o, lse, scale, causal):
+    """Gradients of `_attn_ref`."""
     qf, kf, vf = (t.float().permute(0, 2, 1, 3) for t in (q, k, v))
     dof = do.float().permute(0, 2, 1, 3)
     of = o.float().permute(0, 2, 1, 3)
@@ -461,11 +478,6 @@ def attention_bwd(do: Tensor, q: Tensor, k: Tensor, v: Tensor, o: Tensor, lse: T
     dq = torch.matmul(ds, kf)
     dk = torch.matmul(ds.transpose(-1, -2), qf)
     return tuple(t.permute(0, 2, 1, 3).contiguous().to(q.dtype) for t in (dq, dk, dv))
-
-
-@attention_bwd.register_fake
-def _(do, q, k, v, o, lse, scale, causal):
-    return (q.new_empty(q.shape), k.new_empty(k.shape), v.new_empty(v.shape))
 
 
 def _attn_setup(ctx, inputs, output):
@@ -497,11 +509,6 @@ def _gqa_split(qkv):
     return qkv[:, :, :, :G], qkv[:, :, :, G], qkv[:, :, :, G + 1]
 
 
-def _gqa_native(qkv: Tensor, *others: Tensor) -> bool:
-    return (uses_native(qkv, *others) and qkv.shape[3] > 2 and qkv.shape[-1] % 8 == 0 and qkv.shape[-1] <= 128
-            and qkv.stride(-1) == 1)
-
-
 def _gqa_expand(q, k, v):
     """q [B,Sq,Hkv,G,D], k / v [B,Skv,Hkv,D] -> [B,S,Hkv*G,D] each, K/V repeated per query head."""
     B, Sq, Hkv, G, D = q.shape
@@ -521,7 +528,7 @@ def _gqa_attn_ref_bwd(do, q, k, v, o, lse, scale, causal):
     """Gradients of `_gqa_attn_ref`: dq like q, dk / dv like k / v (summed over each group in fp32)."""
     B, Sq, Hkv, G, D = q.shape
     Hq = Hkv * G
-    dq, dk, dv = attention_bwd(do.reshape(B, Sq, Hq, D), *_gqa_expand(q, k, v), o.reshape(B, Sq, Hq, D),
+    dq, dk, dv = _attn_ref_bwd(do.reshape(B, Sq, Hq, D), *_gqa_expand(q, k, v), o.reshape(B, Sq, Hq, D),
                                lse.reshape(B, Hq, Sq), scale, causal)
     group_sum = lambda t: t.view(B, -1, Hkv, G, D).float().sum(3).to(q.dtype)  # noqa: E731
     return dq.view(B, Sq, Hkv, G, D), group_sum(dk), group_sum(dv)
@@ -532,8 +539,10 @@ def attention_gqa_packed(qkv: Tensor, scale: float, causal: bool) -> Tuple[Tenso
     """(o [B,S,Hkv,G,D], lse [B,Hkv,G,S]) = grouped-query softmax attention of qkv [B,S,Hkv,G+2,D].  G = 1 is
     multi-head attention."""
     q, k, v = _gqa_split(qkv)
-    if _gqa_native(qkv):
-        o, lse = _native().attention_fwd(q, k, v, scale, causal)
+    D = qkv.shape[-1]
+    if C := _kernels("attention_gqa_packed", qkv,
+                     unsupported=_attn_unsupported(D, qkv.stride(-1)) or (None if q.shape[3] else "empty query group")):
+        o, lse = C.attention_fwd(q, k, v, scale, causal)
         return o, lse
     return _gqa_attn_ref(q, k, v, scale, causal)
 
@@ -548,11 +557,11 @@ def _(qkv, scale, causal):
 def attention_gqa_packed_bwd(do: Tensor, qkv: Tensor, o: Tensor, lse: Tensor, scale: float, causal: bool) -> Tensor:
     """dqkv [B,S,Hkv,G+2,D]: dQ in slots 0..G-1, dK (summed over the group) in slot G, dV in slot G + 1"""
     q, k, v = _gqa_split(qkv)
-    G = q.shape[3]
+    G, D = q.shape[3], qkv.shape[-1]
     dqkv = torch.empty(qkv.shape, device=qkv.device, dtype=qkv.dtype)
-    if _gqa_native(qkv, do, o):
-        _native().attention_bwd(do, q, k, v, o, lse, scale, causal, dqkv[:, :, :, :G], dqkv[:, :, :, G],
-                                dqkv[:, :, :, G + 1])
+    if C := _kernels("attention_gqa_packed_bwd", qkv, do, o,
+                     unsupported=_attn_unsupported(D, qkv.stride(-1)) or (None if G else "empty query group")):
+        C.attention_bwd(do, q, k, v, o, lse, scale, causal, dqkv[:, :, :, :G], dqkv[:, :, :, G], dqkv[:, :, :, G + 1])
         return dqkv
     dqkv[:, :, :, :G], dqkv[:, :, :, G], dqkv[:, :, :, G + 1] = _gqa_attn_ref_bwd(do, q, k, v, o, lse, scale, causal)
     return dqkv
@@ -589,8 +598,8 @@ attention_gqa_packed.register_autograd(_attn_gqa_bwd, setup_context=_attn_packed
 def embedding(ids: Tensor, wte: Tensor, vocab_start: int = 0) -> Tensor:
     """x[..., H] = wte[ids - vocab_start] (zeros for ids outside this vocab shard)"""
     V = wte.shape[0]
-    if uses_native(wte) and wte.shape[1] % 8 == 0:
-        return _native().embedding_fwd(ids.contiguous(), None, wte.contiguous(), None, vocab_start)
+    if C := _kernels("embedding", wte, unsupported=None if wte.shape[1] % 8 == 0 else "H not a multiple of 8"):
+        return C.embedding_fwd(ids.contiguous(), None, wte.contiguous(), None, vocab_start)
     local = ids - vocab_start
     ok = (local >= 0) & (local < V)
     out = F.embedding(local.clamp(0, V - 1), wte)
@@ -606,9 +615,9 @@ def _(ids, wte, vocab_start=0):
 def embedding_bwd(ids: Tensor, dy: Tensor, num_rows: int, vocab_start: int = 0) -> Tensor:
     """dwte[num_rows, H] = scatter-add of dy rows at (ids - vocab_start)"""
     H = dy.shape[-1]
-    if uses_native(dy) and H % 2 == 0:
+    if C := _kernels("embedding_bwd", dy, unsupported=None if H % 2 == 0 else "odd H"):
         dt = torch.zeros(num_rows, H, device=dy.device, dtype=torch.float32)
-        _native().embedding_bwd_(ids.contiguous(), dy.contiguous(), dt, vocab_start)
+        C.embedding_bwd_(ids.contiguous(), dy.contiguous(), dt, vocab_start)
         return dt.to(dy.dtype)
     local = (ids - vocab_start).reshape(-1)
     ok = (local >= 0) & (local < num_rows)
@@ -644,28 +653,18 @@ embedding.register_autograd(_emb_bwd, setup_context=_emb_setup)
 # =================================================================================================
 # decode attention over a KV cache whose valid length lives on the device (serving; not differentiable)
 # =================================================================================================
-def attention_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, kv_len: Tensor, scale: float) -> Tensor:
-    """q: [B, T, h, D] (the last T positions); k/v_cache: [B, S_max, h, D]; kv_len: int32 scalar tensor = number of
-    valid cache rows (including the T new ones).  Causal inside the new block.  Because the length is read on the
-    device, one captured CUDA graph serves every decode position."""
-    if uses_native(q, k_cache, v_cache):
-        return _native().attention_fwd(q if q.stride(-1) == 1 else q.contiguous(), k_cache, v_cache, scale, True,
-                                       kv_len)[0]
-    n = int(kv_len)
-    return _attn_ref(q, k_cache[:, :n], v_cache[:, :n], scale, True)[0]
-
-
 def decode_attention(q: Tensor, k_new: Tensor, v_new: Tensor, k_cache: Tensor, v_cache: Tensor, kv_len: Tensor,
                      scale: float) -> Tensor:
     """One new token per sequence with the cache append fused in.  q / k_new / v_new: [B, 1, h, D] (views of the fused
     QKV projection are fine); k/v_cache: [B, S_max, h, D], updated in place at row kv_len-1; kv_len: int32 scalar tensor
-    = valid rows including the new one.  Returns o [B, 1, h, D].  Replaces two strided copies, two index_copy launches
-    and the padded tensor-core attention of `attention_decode` with one cache-streaming kernel."""
-    if uses_native(q, k_cache, v_cache) and hasattr(_native(), "decode_attention"):
+    = valid rows including the new one; because it is read on the device, one captured CUDA graph serves every decode
+    position.  Returns o [B, 1, h, D].  One cache-streaming kernel: no separate cache copies, no padded tensor-core
+    attention."""
+    if C := _kernels("decode_attention", q, k_cache, v_cache):
         if k_new.stride() != v_new.stride() or k_new.stride(-1) != 1:      # e.g. k went through rotary, v did not
             k_new, v_new = k_new.contiguous(), v_new.contiguous()
-        return _native().decode_attention(q if q.stride(-1) == 1 else q.contiguous(), k_new, v_new, k_cache, v_cache,
-                                          kv_len, scale)
+        return C.decode_attention(q if q.stride(-1) == 1 else q.contiguous(), k_new, v_new, k_cache, v_cache, kv_len,
+                                  scale)
     n = int(kv_len)
     k_cache[:, n - 1:n] = k_new
     v_cache[:, n - 1:n] = v_new
@@ -700,21 +699,18 @@ def attention_cached_(q: Tensor, k_new: Tensor, v_new: Tensor, k_cache: Tensor, 
                       scale: float) -> Tensor:
     """In-place form of `attention_cached`: k/v_cache are updated, o is returned."""
     T = q.shape[1]
-    if uses_native(q, k_cache, v_cache) and q.shape[-1] % 8 == 0 and q.shape[-1] <= 128:
-        if T == 1 and hasattr(_native(), "decode_attention"):
-            kv_len = (cache_len.to(torch.int32) + 1).reshape(())
-            return decode_attention(q, k_new, v_new, k_cache, v_cache, kv_len, scale)
-        # prompt chunk: same kernel path as the serving decoder's prefill (flash attention over the valid cache rows,
-        # causal with Sq != Sk); the length is read on the host here -- only the T = 1 step has to be sync-free
-        n0 = int(cache_len)
-        k_cache[:, n0:n0 + T] = k_new
-        v_cache[:, n0:n0 + T] = v_new
-        return attention(q if q.stride(-1) == 1 else q.contiguous(), k_cache[:, :n0 + T], v_cache[:, :n0 + T], scale,
-                         True)[0]
+    C = _kernels("attention_cached", q, k_cache, v_cache, unsupported=_attn_unsupported(q.shape[-1]))
+    if C is not None and T == 1:
+        return decode_attention(q, k_new, v_new, k_cache, v_cache, (cache_len.to(torch.int32) + 1).reshape(()), scale)
+    # prompt chunk: same kernel path as the serving decoder's prefill (flash attention over the valid cache rows,
+    # causal with Sq != Sk); the length is read on the host here -- only the T = 1 step has to be sync-free
     n0 = int(cache_len)
     k_cache[:, n0:n0 + T] = k_new
     v_cache[:, n0:n0 + T] = v_new
-    return _attn_ref(q, k_cache[:, :n0 + T], v_cache[:, :n0 + T], scale, True)[0]
+    k, v = k_cache[:, :n0 + T], v_cache[:, :n0 + T]
+    if C is None:
+        return _attn_ref(q, k, v, scale, True)[0]
+    return attention(q if q.stride(-1) == 1 else q.contiguous(), k, v, scale, True)[0]       # the kernel reads D rows
 
 
 # =================================================================================================
@@ -725,9 +721,9 @@ def ragged_attention(q: Tensor, k_cache: Tensor, v_cache: Tensor, seq_start: Ten
     """q: [T, h, D]; k/v_cache: [slots, h, D]; token t attends to cache rows seq_start[t] .. seq_start[t]+ctx_len[t]-1
     (ctx_len 0 = padding token -> zeros).  `max_ctx` bounds ctx_len (sizes the score buffer).  `alibi`: optional fp32
     [h] slopes, bias = slope * key position.  (reference: the external fused_mmha of opt_model_1d.py:151-178)"""
-    if uses_native(q, k_cache, v_cache):
-        return _native().ragged_attention(q if q.stride(-1) == 1 else q.contiguous(), k_cache, v_cache, seq_start,
-                                          ctx_len, scale, max_ctx, alibi)
+    if C := _kernels("ragged_attention", q, k_cache, v_cache):
+        return C.ragged_attention(q if q.stride(-1) == 1 else q.contiguous(), k_cache, v_cache, seq_start, ctx_len,
+                                  scale, max_ctx, alibi)
     T, h, D = q.shape
     longest = int(ctx_len.max()) if T else 0
     if longest > max_ctx:
@@ -797,9 +793,9 @@ def dropout(x: Tensor, p: float, seed: Tensor, stream: int, global_shape: List[i
     (reference: stateful XLA RNG with per-device seeds, alpa/monkey_patch.py:52-160)"""
     if p <= 0.0:
         return x.clone()
-    if x.is_cuda and 1 <= x.dim() <= 6 and x.dtype in (torch.bfloat16, torch.float32) and \
-            (uses_native(x) or (x.dtype == torch.float32 and uses_native(x.new_empty(0, dtype=torch.bfloat16)))):
-        return _native().dropout(x, float(p), seed.to(x.device), int(stream), list(global_shape), list(offsets))
+    if C := _kernels("dropout", x, dtypes=(torch.bfloat16, torch.float32),
+                     unsupported=None if 1 <= x.dim() <= 6 else "rank outside 1..6"):
+        return C.dropout(x, float(p), seed.to(x.device), int(stream), list(global_shape), list(offsets))
     keep = dropout_keep_mask(tuple(x.shape), p, seed, stream, global_shape, offsets, device=x.device)
     return torch.where(keep, x.float() * (1.0 / (1.0 - p)), torch.zeros((), device=x.device)).to(x.dtype)
 
@@ -841,23 +837,23 @@ def linear_decode(x: Tensor, w: Tensor, w_scale: Optional[Tensor], b: Optional[T
     kernel's prologue (one launch less per projection); None = x is used as is."""
     rows = x.numel() // x.shape[-1]
     K = x.shape[-1]
-    if x.is_cuda and global_config.use_native_kernels and rows <= 8 and x.dtype == torch.bfloat16:
-        from alpa_b200 import ops
-        fp8w = w.dtype == torch.float8_e4m3fn
-        if ops.native_available() and hasattr(_native(), "gemv_decode") and K % (64 if fp8w else 32) == 0 and \
-                rows * K * (1 if fp8w else 2) <= 200 * 1024:
-            x2 = _as2d(x)
-            if x2.stride(0) % 8 or x2.data_ptr() % 16:     # the prologue reads rows 16 bytes at a time
-                x2 = x2.contiguous()
-            r2 = None if residual is None else _as2d(residual)
-            if ln is not None and ln[0].dtype != torch.bfloat16:
-                x2 = layer_norm(x2, ln[0], ln[1], ln[2])[0]          # the fused prologue reads bf16 gamma / beta
-                ln = None
-            if ln is None:
-                y = _native().gemv_decode(x2, w, w_scale, b, r2, _ACT_IDS[act])
-            else:
-                y = _native().gemv_decode(x2, w, w_scale, b, r2, _ACT_IDS[act], ln[0], ln[1], float(ln[2]))
-            return y.view(*x.shape[:-1], w.shape[0])
+    fp8w = w.dtype == torch.float8_e4m3fn
+    unsupported = ("more than 8 rows" if rows > 8 else
+                   "K not a multiple of the GEMV's K step" if K % (64 if fp8w else 32) else
+                   "staged activations over 200 KiB" if rows * K * (1 if fp8w else 2) > 200 * 1024 else None)
+    if C := _kernels("linear_decode", x, unsupported=unsupported):          # the binding checks w: bf16 or e4m3
+        x2 = _as2d(x)
+        if x2.stride(0) % 8 or x2.data_ptr() % 16:     # the prologue reads rows 16 bytes at a time
+            x2 = x2.contiguous()
+        r2 = None if residual is None else _as2d(residual)
+        if ln is not None and ln[0].dtype != torch.bfloat16:
+            x2 = layer_norm(x2, ln[0], ln[1], ln[2])[0]          # the fused prologue reads bf16 gamma / beta
+            ln = None
+        if ln is None:
+            y = C.gemv_decode(x2, w, w_scale, b, r2, _ACT_IDS[act])
+        else:
+            y = C.gemv_decode(x2, w, w_scale, b, r2, _ACT_IDS[act], ln[0], ln[1], float(ln[2]))
+        return y.view(*x.shape[:-1], w.shape[0])
     if ln is not None:
         x = F.layer_norm(x.float(), (K,), ln[0].float(), ln[1].float(), ln[2]).to(x.dtype)
     wf = w.to(torch.float32) * w_scale[:, None] if w_scale is not None else w.to(torch.float32)
@@ -871,14 +867,12 @@ def linear_fp8(x: Tensor, w_fp8: Tensor, w_scale: Tensor, b: Optional[Tensor] = 
     """y = act(x @ (w_fp8 * w_scale[:, None])^T + b).  On sm_90a the activations are quantised per token to e4m3
     and the product runs on the fp8 tensor cores (`kind::f8f6f4`), scales applied in the epilogue; elsewhere the
     weights are dequantised (same maths up to the activation rounding)."""
-    if x.is_cuda and global_config.use_native_kernels:
-        from alpa_b200 import ops
-        if ops.native_available() and hasattr(_native(), "gemm_fp8") and x.shape[-1] % 16 == 0 and w_fp8.shape[0] % 8 == 0:
-            x2 = _as2d(x)
-            if x2.stride(0) % 8 or x2.data_ptr() % 16:     # the quantiser reads rows 16 bytes at a time
-                x2 = x2.contiguous()
-            y = _native().gemm_fp8(x2, w_fp8, w_scale, b, _ACT_IDS[act])
-            return y.view(*x.shape[:-1], w_fp8.shape[0])
+    if C := _kernels("linear_fp8", x, unsupported=None if x.shape[-1] % 16 == 0 and w_fp8.shape[0] % 8 == 0
+                     else "K % 16 or N % 8"):
+        x2 = _as2d(x)
+        if x2.stride(0) % 8 or x2.data_ptr() % 16:     # the quantiser reads rows 16 bytes at a time
+            x2 = x2.contiguous()
+        return C.gemm_fp8(x2, w_fp8, w_scale, b, _ACT_IDS[act]).view(*x.shape[:-1], w_fp8.shape[0])
     w = (w_fp8.to(torch.float32) * w_scale[:, None]).to(x.dtype)
     y = F.linear(x, w, b)
     return _act_fn(y, act)
@@ -892,17 +886,20 @@ def packed_nbytes(views: List[Tensor]) -> int:
     return sum((v.numel() * v.element_size() + 15) // 16 * 16 for v in views)
 
 
-def _pack_native_ok(views: List[Tensor], flat: Tensor) -> bool:
-    return (flat.is_cuda and global_config.use_native_kernels and hasattr(_native(), "pack_tiles") and
-            all(v.is_cuda and 1 <= v.dim() <= 4 and v.stride(-1) == 1 and v.numel() > 0 for v in views))
+def _tiles_unsupported(views: List[Tensor]) -> Optional[str]:
+    """Why the pack kernel cannot move these tiles (non-empty, 1-D to 4-D, rows contiguous), or None."""
+    ok = all(1 <= v.dim() <= 4 and v.stride(-1) == 1 and v.numel() > 0 for v in views)
+    return None if ok else "tile empty, over 4-D or with strided rows"
 
 
 def pack_tiles(views: List[Tensor], flat: Optional[Tensor] = None) -> Tensor:
     """Gather strided slices into one uint8 staging buffer (one launch on sm_90a: pack_sm90.cu)."""
     if flat is None:
         flat = torch.empty(packed_nbytes(views), dtype=torch.uint8, device=views[0].device)
-    if views and _pack_native_ok(views, flat):
-        _native().pack_tiles(list(views), flat, False)
+    C = _kernels("pack_tiles", flat, *views, dtypes=None,
+                 unsupported=lambda: _tiles_unsupported(views)) if views else None
+    if C is not None:
+        C.pack_tiles(list(views), flat, False)
         return flat
     off = 0
     for v in views:
@@ -914,8 +911,10 @@ def pack_tiles(views: List[Tensor], flat: Optional[Tensor] = None) -> Tensor:
 
 def unpack_tiles(flat: Tensor, views: List[Tensor]) -> None:
     """Scatter a received staging buffer into the destination slices (in place)."""
-    if views and _pack_native_ok(views, flat):
-        _native().pack_tiles(list(views), flat, True)
+    C = _kernels("unpack_tiles", flat, *views, dtypes=None,
+                 unsupported=lambda: _tiles_unsupported(views)) if views else None
+    if C is not None:
+        C.pack_tiles(list(views), flat, True)
         return
     off = 0
     for v in views:
@@ -971,9 +970,9 @@ def _quantize_mxfp8_ref(x: Tensor) -> Tuple[Tensor, Tensor]:
 def quantize_mxfp8(x: Tensor) -> Tuple[Tensor, Tensor]:
     """x [rows, K] (K % 32 == 0) -> (q e4m3 [rows, K], scale atoms uint8 [ceil(rows/128), ceil(K/128), 512])."""
     assert x.dim() == 2 and x.shape[1] % MX_BLOCK == 0, "quantize_mxfp8: [rows, K] with K % 32 == 0"
-    if uses_native(x) and hasattr(_native(), "quantize_mxfp8"):
+    if C := _kernels("quantize_mxfp8", x):
         ok = x.stride(-1) == 1 and x.stride(0) % 8 == 0 and x.data_ptr() % 16 == 0
-        q, sf = _native().quantize_mxfp8(x if ok else x.contiguous())
+        q, sf = C.quantize_mxfp8(x if ok else x.contiguous())
         return q, sf
     return _quantize_mxfp8_ref(x)
 
@@ -991,11 +990,10 @@ def linear_mxfp8(x: Tensor, w_q: Tensor, w_sf: Tensor, b: Optional[Tensor] = Non
     memory); elsewhere both operands are dequantised -- the same maths, activation rounding included."""
     K, N = x.shape[-1], w_q.shape[0]
     x2 = _as2d(x)
-    if uses_native(x) and hasattr(_native(), "gemm_mxfp8") and K % MX_BLOCK == 0 and N % 8 == 0:
+    if C := _kernels("linear_mxfp8", x, unsupported=None if K % MX_BLOCK == 0 and N % 8 == 0 else "K % 32 or N % 8"):
         if x2.stride(0) % 8 or x2.data_ptr() % 16:         # the quantiser reads rows 16 bytes at a time
             x2 = x2.contiguous()
-        y = _native().gemm_mxfp8(x2, w_q, w_sf, b, _ACT_IDS[act])
-        return y.view(*x.shape[:-1], N)
+        return C.gemm_mxfp8(x2, w_q, w_sf, b, _ACT_IDS[act]).view(*x.shape[:-1], N)
     xq, x_sf = _quantize_mxfp8_ref(x2)
     y = F.linear(dequantize_mxfp8(xq, x_sf), dequantize_mxfp8(w_q, w_sf), None if b is None else b.float())
     return _act_fn(y, act).to(x.dtype).view(*x.shape[:-1], N)
@@ -1008,8 +1006,8 @@ def linear_mxfp8(x: Tensor, w_q: Tensor, w_sf: Tensor, b: Optional[Tensor] = Non
 @torch.library.custom_op("alpa_b200::bmm", mutates_args=())
 def bmm(a: Tensor, b: Tensor, trans_a: bool, trans_b: bool) -> Tensor:
     """C[B, M, N] = op(a) @ op(b)^T-convention (see above)"""
-    if uses_native(a, b) and _gemm_ok(a, b):
-        return _native().gemm(a, b, trans_a, trans_b)
+    if C := _kernels("bmm", a, b, unsupported=lambda: _gemm_unsupported(a, b)):
+        return C.gemm(a, b, trans_a, trans_b)
     am = a.transpose(-1, -2) if trans_a else a
     bm = b if trans_b else b.transpose(-1, -2)
     return torch.matmul(am, bm)
@@ -1057,24 +1055,20 @@ def moe_top2_route(gates: Tensor, capacity: int) -> Tuple[Tensor, Tensor]:
     -> (expert [G,S,2], slot [G,S,2]) int64.  First choices fill an expert's capacity in token order, second
     choices continue after them; slot = -1 when the expert is full."""
     G, S, E = gates.shape
-    C = capacity
-    if gates.is_cuda and global_config.use_native_kernels:
-        from alpa_b200 import ops
-        if ops.native_available():
-            return tuple(_native().moe_top2_route(gates.float().contiguous(), C))
-        if not ops.allow_fallback():
-            raise RuntimeError("alpa_b200: sm_90a extension missing for moe_top2_route")
+    C = _kernels("moe_top2_route", gates, dtypes=None)     # the kernel reads the gates as fp32
+    if C is not None:
+        return tuple(C.moe_top2_route(gates.float().contiguous(), capacity))
     idx1 = gates.argmax(-1)
     mask1 = F.one_hot(idx1, E)
     idx2 = (gates * (1 - mask1)).argmax(-1)
     mask2 = F.one_hot(idx2, E)
     pos1_all = mask1.cumsum(-2) - mask1
-    keep1 = (pos1_all < C) & mask1.bool()
+    keep1 = (pos1_all < capacity) & mask1.bool()
     pos1 = (pos1_all * keep1).sum(-1)
     ok1 = keep1.any(-1)
     count1 = keep1.sum(-2)
     pos2_all = (mask2.cumsum(-2) - mask2) + count1.unsqueeze(-2)
-    keep2 = (pos2_all < C) & mask2.bool()
+    keep2 = (pos2_all < capacity) & mask2.bool()
     pos2 = (pos2_all * keep2).sum(-1)
     ok2 = keep2.any(-1)
     expert = torch.stack([idx1, idx2], -1)
@@ -1095,10 +1089,10 @@ def moe_dispatch(x: Tensor, expert: Tensor, slot: Tensor, weight: Optional[Tenso
     """d[e, g*C+c, :] = (weight[g,s,k] *) x[g,s,:] for every routed (g,s,k); zeros in unused slots"""
     G, S, M = x.shape
     K = expert.shape[-1]
-    if uses_native(x, weight) and M % 8 == 0:
+    if C := _kernels("moe_dispatch", x, weight, unsupported=None if M % 8 == 0 else "M not a multiple of 8"):
         d = torch.zeros(num_experts, G * capacity, M, device=x.device, dtype=x.dtype)
-        _native().moe_dispatch_(x.contiguous(), expert.contiguous(), slot.contiguous(),
-                                None if weight is None else weight.contiguous(), d, capacity)
+        C.moe_dispatch_(x.contiguous(), expert.contiguous(), slot.contiguous(),
+                        None if weight is None else weight.contiguous(), d, capacity)
         return d
     d = torch.zeros(num_experts * G * capacity + 1, M, device=x.device, dtype=x.dtype)
     g = torch.arange(G, device=x.device).view(G, 1, 1)
@@ -1121,13 +1115,13 @@ def moe_combine(eo: Tensor, expert: Tensor, slot: Tensor, weight: Optional[Tenso
     """out[g,s,:] = sum_k weight[g,s,k] * eo[expert[g,s,k], g*C + slot[g,s,k], :]  (weight=None: 1)"""
     E, GC, M = eo.shape
     G, S, K = expert.shape
-    C = GC // G
-    if uses_native(eo, weight) and M % 8 == 0:
-        return _native().moe_combine(eo.contiguous(), expert.contiguous(), slot.contiguous(),
-                                     None if weight is None else weight.contiguous())
+    cap = GC // G
+    if C := _kernels("moe_combine", eo, weight, unsupported=None if M % 8 == 0 else "M not a multiple of 8"):
+        return C.moe_combine(eo.contiguous(), expert.contiguous(), slot.contiguous(),
+                             None if weight is None else weight.contiguous())
     g = torch.arange(G, device=eo.device).view(G, 1, 1)
     ok = slot >= 0
-    row = torch.where(ok, (expert * G + g) * C + slot, torch.zeros_like(slot))
+    row = torch.where(ok, (expert * G + g) * cap + slot, torch.zeros_like(slot))
     rows = eo.reshape(E * GC, M)[row.reshape(-1)].view(G, S, K, M).float()
     w = ok.float() if weight is None else weight.float() * ok.float()
     return (rows * w.unsqueeze(-1)).sum(2).to(eo.dtype)
@@ -1144,13 +1138,12 @@ def moe_combine_wgrad(dout: Tensor, eo: Tensor, expert: Tensor, slot: Tensor) ->
     """dweight[g,s,k] = <dout[g,s,:], eo[expert, g*C+slot, :]> (0 for dropped choices)"""
     E, GC, M = eo.shape
     G, S, K = expert.shape
-    C = GC // G
-    if uses_native(eo, dout) and M % 8 == 0:
-        return _native().moe_combine_wgrad(dout.contiguous(), eo.contiguous(), expert.contiguous(),
-                                           slot.contiguous())
+    cap = GC // G
+    if C := _kernels("moe_combine_wgrad", eo, dout, unsupported=None if M % 8 == 0 else "M not a multiple of 8"):
+        return C.moe_combine_wgrad(dout.contiguous(), eo.contiguous(), expert.contiguous(), slot.contiguous())
     g = torch.arange(G, device=eo.device).view(G, 1, 1)
     ok = slot >= 0
-    row = torch.where(ok, (expert * G + g) * C + slot, torch.zeros_like(slot))
+    row = torch.where(ok, (expert * G + g) * cap + slot, torch.zeros_like(slot))
     rows = eo.reshape(E * GC, M)[row.reshape(-1)].view(G, S, K, M).float()
     dw = (rows * dout.float().unsqueeze(2)).sum(-1) * ok.float()
     return dw.to(dout.dtype)
@@ -1215,8 +1208,9 @@ def cross_entropy(logits: Tensor, labels: Tensor, vocab_start: int = 0) -> Tuple
     V = logits.shape[-1]
     l2 = logits.reshape(T, V)
     lab = labels.reshape(T)
-    if uses_native(logits) and V % 8 == 0 and l2.stride(0) % 8 == 0 and l2.stride(1) == 1:
-        stats = _native().ce_stats(l2, lab.contiguous(), vocab_start)
+    aligned = V % 8 == 0 and l2.stride(0) % 8 == 0 and l2.stride(1) == 1
+    if C := _kernels("cross_entropy", logits, unsupported=None if aligned else "vocab rows not 16-byte aligned"):
+        stats = C.ce_stats(l2, lab.contiguous(), vocab_start)
     else:
         lf = l2.float()
         mx = lf.max(dim=1).values
@@ -1241,10 +1235,9 @@ def cross_entropy_bwd(logits: Tensor, labels: Tensor, stats: Tensor, dloss: Tens
     T = labels.numel()
     V = logits.shape[-1]
     lab = labels.reshape(T)
-    if uses_native(logits) and V % 8 == 0:
+    if C := _kernels("cross_entropy_bwd", logits, unsupported=None if V % 8 == 0 else "V not a multiple of 8"):
         g = logits.reshape(T, V).clone()
-        _native().ce_grad_(g, lab.contiguous(), stats[:, :2].contiguous(),
-                           dloss.reshape(T).float().contiguous(), vocab_start)
+        C.ce_grad_(g, lab.contiguous(), stats[:, :2].contiguous(), dloss.reshape(T).float().contiguous(), vocab_start)
         return g.view(logits.shape)
     lf = logits.reshape(T, V).float()
     p = torch.exp(lf - stats[:, 0:1]) / stats[:, 1:2]
@@ -1292,35 +1285,32 @@ def fused_adamw_(params: List[Tensor], masters: List[Tensor], ms: List[Tensor], 
     """`step` is the 1-based step count as a scalar tensor (read on the device by the kernel).
     One launch updates every parameter: master -= lr * (m_hat / (sqrt(v_hat)+eps) + wd * master);
     params (bf16 compute copies, may alias masters when training in fp32) are refreshed in the same pass."""
-    if masters and masters[0].is_cuda and global_config.use_native_kernels:
-        from alpa_b200 import ops
-        if ops.native_available() and all(g.dtype in (torch.float32, torch.bfloat16) for g in grads):
-            # Non-contiguous gradients are copied into persistent contiguous staging buffers every step (the
-            # device table points at the staging buffer, which the cache entry keeps alive).
-            key = tuple((t.data_ptr(), t.numel(), t.dtype, t.is_contiguous())
-                        for t in (*grads, *masters, *ms, *vs, *params)) + tuple(weight_decays)
-            ent = _adam_table_cache.get(key)
-            if ent is None:
-                pb = [p if (p.dtype == torch.bfloat16 and p.data_ptr() != m.data_ptr()) else None
-                      for p, m in zip(params, masters)]
-                staging = [None if g.is_contiguous() else torch.empty(g.shape, dtype=g.dtype, device=g.device)
-                           for g in grads]
-                gsrc = [g if st is None else st for g, st in zip(grads, staging)]
-                tab = _native().adam_build_tables(gsrc, masters, ms, vs, pb, list(weight_decays))
-                if len(_adam_table_cache) > 64:
-                    _adam_table_cache.clear()
-                # the entry owns the staging buffers and the optimizer state the table points at; gradients are looked
-                # up by (address, numel, dtype), so a recycled address holding an identically shaped gradient is the
-                # same table and anything else is a different key (holding the gradients themselves would pin them)
-                ent = (tab, staging, (list(masters), list(ms), list(vs), list(params)))
-                _adam_table_cache[key] = ent
-            tab, staging = ent[0], ent[1]
-            for g, st in zip(grads, staging):
-                if st is not None:
-                    st.copy_(g)
-            _native().adamw_step(tab[0], tab[1], lr, beta1, beta2, eps, 1, grad_scale, None,
-                                 step.float().reshape(1))
-            return
+    if C := _kernels("fused_adamw_", *masters, *grads, dtypes=(torch.float32, torch.bfloat16)):
+        # Non-contiguous gradients are copied into persistent contiguous staging buffers every step (the
+        # device table points at the staging buffer, which the cache entry keeps alive).
+        key = tuple((t.data_ptr(), t.numel(), t.dtype, t.is_contiguous())
+                    for t in (*grads, *masters, *ms, *vs, *params)) + tuple(weight_decays)
+        ent = _adam_table_cache.get(key)
+        if ent is None:
+            pb = [p if (p.dtype == torch.bfloat16 and p.data_ptr() != m.data_ptr()) else None
+                  for p, m in zip(params, masters)]
+            staging = [None if g.is_contiguous() else torch.empty(g.shape, dtype=g.dtype, device=g.device)
+                       for g in grads]
+            gsrc = [g if st is None else st for g, st in zip(grads, staging)]
+            tab = C.adam_build_tables(gsrc, masters, ms, vs, pb, list(weight_decays))
+            if len(_adam_table_cache) > 64:
+                _adam_table_cache.clear()
+            # the entry owns the staging buffers and the optimizer state the table points at; gradients are looked
+            # up by (address, numel, dtype), so a recycled address holding an identically shaped gradient is the
+            # same table and anything else is a different key (holding the gradients themselves would pin them)
+            ent = (tab, staging, (list(masters), list(ms), list(vs), list(params)))
+            _adam_table_cache[key] = ent
+        tab, staging = ent[0], ent[1]
+        for g, st in zip(grads, staging):
+            if st is not None:
+                st.copy_(g)
+        C.adamw_step(tab[0], tab[1], lr, beta1, beta2, eps, 1, grad_scale, None, step.float().reshape(1))
+        return
     stepf = float(step)
     bc1 = 1.0 - beta1 ** stepf
     bc2 = 1.0 - beta2 ** stepf
@@ -1392,11 +1382,12 @@ DIRECT_IMPL, _fast_ns = _collect_direct()
 
 def _linear_wgrad_out(dy: Tensor, x: Tensor, out: Tensor) -> Tensor:
     """linear_wgrad writing dw straight into `out` (a slice of a gradient bucket): no pack copy before the collective."""
-    if uses_native(dy, x) and out.dtype == torch.bfloat16:
-        d2, x2 = _as2d(dy), _as2d(x)
-        if _gemm_ok(d2, x2) and out.stride(-1) == 1 and out.data_ptr() % 16 == 0 and out.stride(0) % 8 == 0:
-            _native().gemm(d2, x2, True, True, out=out)
-            return out
+    v = cache(lambda: (_as2d(dy), _as2d(x)))
+    # an `out` the epilogue cannot store to directly is no fallback: linear_wgrad runs and its result is copied
+    out_ok = out.dtype == torch.bfloat16 and out.stride(-1) == 1 and out.data_ptr() % 16 == 0 and out.stride(0) % 8 == 0
+    if out_ok and (C := _kernels("linear_wgrad", dy, x, unsupported=lambda: _gemm_unsupported(*v()))):
+        C.gemm(*v(), True, True, out=out)
+        return out
     out.copy_(linear_wgrad._init_fn(dy, x))
     return out
 
@@ -1419,7 +1410,6 @@ class _FastNamespace:
         self.__dict__.update(fns)
         self.linear_fp8 = linear_fp8
         self.linear_decode = linear_decode
-        self.attention_decode = attention_decode
         self.decode_attention = decode_attention
         self.ragged_attention = ragged_attention
         self.linear_mxfp8 = linear_mxfp8
