@@ -451,14 +451,17 @@ int64_t attention_bwd_splits(const Tensor& q, const Tensor& k, const Tensor& v) 
   return ab_attention_bwd_splits(&a);
 }
 
+// rms: RMSNorm (beta must be absent; the returned mean is undefined)
 std::vector<Tensor> layernorm_fwd(const Tensor& x, const OptTensor& residual, const Tensor& gamma,
-                                  const Tensor& beta, double eps, bool want_sum) {
+                                  const OptTensor& beta, double eps, bool want_sum, bool rms) {
   TORCH_CHECK(x.is_contiguous() && x.scalar_type() == at::kBFloat16);
+  const bool has_beta = beta.has_value() && beta->defined();
+  TORCH_CHECK(has_beta != rms, "layernorm_fwd: LayerNorm takes beta, RMSNorm does not");
   c10::cuda::CUDAGuard guard(x.device());
   const int H = (int)x.size(-1);
   const int rows = (int)(x.numel() / H);
   Tensor y = torch::empty_like(x);
-  Tensor mean = torch::empty({rows}, x.options().dtype(at::kFloat));
+  Tensor mean = rms ? Tensor() : torch::empty({rows}, x.options().dtype(at::kFloat));
   Tensor rstd = torch::empty({rows}, x.options().dtype(at::kFloat));
   Tensor sum;
   ab::LayerNormArgs a;
@@ -474,20 +477,24 @@ std::vector<Tensor> layernorm_fwd(const Tensor& x, const OptTensor& residual, co
   a.gamma = bf16_ptr(gamma);
   a.beta = bf16_ptr(beta);
   a.y = reinterpret_cast<__nv_bfloat16*>(y.data_ptr());
-  a.mean = mean.data_ptr<float>();
+  a.mean = rms ? nullptr : mean.data_ptr<float>();
   a.rstd = rstd.data_ptr<float>();
   a.rows = rows;
   a.H = H;
   a.eps = (float)eps;
+  a.rms = rms ? 1 : 0;
   AB_CHECK_RC(ab_layernorm_fwd(&a, cur_stream()), "ab_layernorm_fwd");
   g_launches += 1;
   return {y, mean, rstd, sum.defined() ? sum : Tensor()};
 }
 
-Tensor layernorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& gamma, const Tensor& mean,
-                     const Tensor& rstd, const OptTensor& dres, Tensor dgamma, Tensor dbeta) {
+// rms: backward of the RMSNorm forward (mean and dbeta must be absent)
+Tensor layernorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& gamma, const OptTensor& mean,
+                     const Tensor& rstd, const OptTensor& dres, Tensor dgamma, const OptTensor& dbeta, bool rms) {
   TORCH_CHECK(dy.is_contiguous() && x.is_contiguous());
-  TORCH_CHECK(dgamma.scalar_type() == at::kFloat && dbeta.scalar_type() == at::kFloat);
+  const bool has_mean = mean.has_value() && mean->defined(), has_dbeta = dbeta.has_value() && dbeta->defined();
+  TORCH_CHECK(has_mean != rms && has_dbeta != rms, "layernorm_bwd: LayerNorm takes mean and dbeta, RMSNorm neither");
+  TORCH_CHECK(dgamma.scalar_type() == at::kFloat && (rms || dbeta->scalar_type() == at::kFloat));
   c10::cuda::CUDAGuard guard(x.device());
   const int H = (int)x.size(-1);
   Tensor dx = torch::empty_like(x);
@@ -495,7 +502,7 @@ Tensor layernorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& gamma, con
   a.dy = bf16_ptr(dy);
   a.x = bf16_ptr(x);
   a.gamma = bf16_ptr(gamma);
-  a.mean = mean.data_ptr<float>();
+  a.mean = rms ? nullptr : mean->data_ptr<float>();
   a.rstd = rstd.data_ptr<float>();
   if (dres.has_value() && dres->defined()) {
     TORCH_CHECK(dres->is_contiguous());
@@ -503,14 +510,66 @@ Tensor layernorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& gamma, con
   }
   a.dx = reinterpret_cast<__nv_bfloat16*>(dx.data_ptr());
   a.dgamma = dgamma.data_ptr<float>();
-  a.dbeta = dbeta.data_ptr<float>();
+  a.dbeta = rms ? nullptr : dbeta->data_ptr<float>();
   a.rows = (int)(x.numel() / H);
   a.H = H;
-  Tensor ws = torch::empty({(int64_t)ab_layernorm_bwd_slots(a.rows, H), 2, H}, x.options().dtype(at::kFloat));
+  a.rms = rms ? 1 : 0;
+  Tensor ws = torch::empty({(int64_t)ab_layernorm_bwd_slots(a.rows, H), rms ? 1 : 2, H}, x.options().dtype(at::kFloat));
   a.ws = ws.data_ptr<float>();
   AB_CHECK_RC(ab_layernorm_bwd(&a, cur_stream()), "ab_layernorm_bwd");
-  g_launches += 3;   // row kernel + fixed-order reductions of dgamma and dbeta
+  g_launches += rms ? 2 : 3;   // row kernel + fixed-order reductions of dgamma (and dbeta)
   return dx;
+}
+
+// qkv: [B, S, Hkv, G + 2, D] contiguous bf16; position_ids: [B, S] int64; inv_freq: [D / 2] fp32.  Rotates slots 0..G
+// by +-theta (inverse: -theta, the backward) and copies slot G + 1.
+Tensor rotary_packed(const Tensor& qkv, const Tensor& position_ids, const Tensor& inv_freq, bool inverse) {
+  TORCH_CHECK(qkv.dim() == 5 && qkv.is_contiguous() && qkv.scalar_type() == at::kBFloat16,
+              "rotary_packed: contiguous bf16 [B, S, Hkv, G + 2, D]");
+  TORCH_CHECK(position_ids.scalar_type() == at::kLong && position_ids.is_contiguous() &&
+              position_ids.numel() == qkv.size(0) * qkv.size(1), "rotary_packed: int64 [B, S] position_ids");
+  const int D = (int)qkv.size(4);
+  TORCH_CHECK(inv_freq.scalar_type() == at::kFloat && inv_freq.is_contiguous() && inv_freq.numel() == D / 2,
+              "rotary_packed: fp32 [D / 2] inv_freq");
+  TORCH_CHECK(qkv.is_cuda() && position_ids.device() == qkv.device() && inv_freq.device() == qkv.device(),
+              "rotary_packed: qkv, position_ids and inv_freq must be on one CUDA device");
+  c10::cuda::CUDAGuard guard(qkv.device());
+  Tensor out = torch::empty_like(qkv);
+  AB_CHECK_RC(ab_rotary_packed(bf16_ptr(qkv), reinterpret_cast<__nv_bfloat16*>(out.data_ptr()),
+                               position_ids.data_ptr<int64_t>(), inv_freq.data_ptr<float>(),
+                               (int)(qkv.size(0) * qkv.size(1)), (int)(qkv.size(2) * qkv.size(3)), (int)qkv.size(3), D,
+                               inverse ? 1 : 0, cur_stream()),
+              "ab_rotary_packed");
+  g_launches += 1;
+  return out;
+}
+
+// gu: [..., I, 2] contiguous bf16 (gate, up pairs) -> h [..., I]
+Tensor swiglu_fwd(const Tensor& gu) {
+  TORCH_CHECK(gu.dim() >= 2 && gu.size(-1) == 2 && gu.is_contiguous() && gu.scalar_type() == at::kBFloat16,
+              "swiglu_fwd: contiguous bf16 [..., I, 2]");
+  c10::cuda::CUDAGuard guard(gu.device());
+  auto shape = gu.sizes().vec();
+  shape.pop_back();
+  Tensor h = torch::empty(shape, gu.options());
+  AB_CHECK_RC(ab_swiglu_fwd(bf16_ptr(gu), reinterpret_cast<__nv_bfloat16*>(h.data_ptr()), gu.numel() / 2,
+                            cur_stream()), "ab_swiglu_fwd");
+  g_launches += 1;
+  return h;
+}
+
+// dh: [..., I], gu: [..., I, 2] -> dgu [..., I, 2]
+Tensor swiglu_bwd(const Tensor& dh, const Tensor& gu) {
+  TORCH_CHECK(gu.dim() >= 2 && gu.size(-1) == 2 && gu.is_contiguous() && gu.scalar_type() == at::kBFloat16,
+              "swiglu_bwd: contiguous bf16 [..., I, 2]");
+  TORCH_CHECK(dh.is_contiguous() && dh.scalar_type() == at::kBFloat16 && dh.numel() * 2 == gu.numel(),
+              "swiglu_bwd: contiguous bf16 dh [..., I]");
+  c10::cuda::CUDAGuard guard(gu.device());
+  Tensor dgu = torch::empty_like(gu);
+  AB_CHECK_RC(ab_swiglu_bwd(bf16_ptr(dh), bf16_ptr(gu), reinterpret_cast<__nv_bfloat16*>(dgu.data_ptr()),
+                            gu.numel() / 2, cur_stream()), "ab_swiglu_bwd");
+  g_launches += 1;
+  return dgu;
 }
 
 Tensor ce_stats(const Tensor& logits, const Tensor& labels, int64_t vocab_start) {
@@ -1034,8 +1093,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("lse"), py::arg("scale"), py::arg("causal"), py::arg("dq_out") = py::none(),
         py::arg("dk_out") = py::none(), py::arg("dv_out") = py::none());
   m.def("attention_bwd_splits", &attention_bwd_splits, py::arg("q"), py::arg("k"), py::arg("v"));
-  m.def("layernorm_fwd", &layernorm_fwd);
-  m.def("layernorm_bwd", &layernorm_bwd);
+  m.def("layernorm_fwd", &layernorm_fwd, py::arg("x"), py::arg("residual"), py::arg("gamma"), py::arg("beta"),
+        py::arg("eps"), py::arg("want_sum"), py::arg("rms") = false);
+  m.def("layernorm_bwd", &layernorm_bwd, py::arg("dy"), py::arg("x"), py::arg("gamma"), py::arg("mean"), py::arg("rstd"),
+        py::arg("dres"), py::arg("dgamma"), py::arg("dbeta"), py::arg("rms") = false);
+  m.def("rotary_packed", &rotary_packed, py::arg("qkv"), py::arg("position_ids"), py::arg("inv_freq"),
+        py::arg("inverse"));
+  m.def("swiglu_fwd", &swiglu_fwd);
+  m.def("swiglu_bwd", &swiglu_bwd);
   m.def("ce_stats", &ce_stats);
   m.def("ce_grad_", &ce_grad_);
   m.def("ragged_attention", &ragged_attention, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("seq_start"),

@@ -12,27 +12,30 @@ struct LayerNormArgs {
   const __nv_bfloat16* x = nullptr;
   const __nv_bfloat16* residual = nullptr;  // optional: normalise (x + residual)
   const __nv_bfloat16* gamma = nullptr;
-  const __nv_bfloat16* beta = nullptr;
+  const __nv_bfloat16* beta = nullptr;  // unused (null) when rms
   __nv_bfloat16* y = nullptr;
   __nv_bfloat16* sum_out = nullptr;  // optional: x + residual
-  float* mean = nullptr;
+  float* mean = nullptr;             // unused (null) when rms
   float* rstd = nullptr;
   int rows = 0, H = 0;
   float eps = 1e-5f;
+  int rms = 0;  // RMSNorm: y = x * rsqrt(mean(x^2) + eps) * gamma (no mean, no beta)
 };
 
 struct LayerNormBwdArgs {
   const __nv_bfloat16* dy = nullptr;
   const __nv_bfloat16* x = nullptr;  // the normalised input (x + residual when fused)
   const __nv_bfloat16* gamma = nullptr;
-  const float* mean = nullptr;
+  const float* mean = nullptr;          // unused (null) when rms
   const float* rstd = nullptr;
   const __nv_bfloat16* dres = nullptr;  // optional gradient flowing through the residual branch
   __nv_bfloat16* dx = nullptr;
   float* dgamma = nullptr;  // accumulated (+=)
-  float* dbeta = nullptr;   // accumulated (+=)
-  float* ws = nullptr;      // [ab_layernorm_bwd_slots(rows, H)][2][H] scratch: per-CTA partials of dgamma / dbeta
+  float* dbeta = nullptr;   // accumulated (+=); unused (null) when rms
+  // [ab_layernorm_bwd_slots(rows, H)][2][H] scratch ([..][1][H] when rms): per-CTA partials of dgamma / dbeta
+  float* ws = nullptr;
   int rows = 0, H = 0;
+  int rms = 0;  // backward of the RMSNorm forward
 };
 
 constexpr int kMaxPeersComm = 8;
@@ -198,6 +201,13 @@ int ab_peer_barrier_auto(uint32_t* const* peer_flags, uint32_t* counter, int ran
 int ab_layernorm_fwd(const ab::LayerNormArgs* a, cudaStream_t st);
 int ab_layernorm_bwd(const ab::LayerNormBwdArgs* a, cudaStream_t st);
 int ab_layernorm_bwd_slots(int rows, int H);
+// x / y: [tokens, heads, D] contiguous, heads = Hkv * slots; the last slot of every K/V head (V) is copied unrotated
+int ab_rotary_packed(const __nv_bfloat16* x, __nv_bfloat16* y, const int64_t* pos, const float* inv_freq, int tokens,
+                     int heads, int slots, int D, int inverse, cudaStream_t st);
+// gu: [pairs, 2] (gate, up); h / dh: [pairs]
+int ab_swiglu_fwd(const __nv_bfloat16* gu, __nv_bfloat16* h, long long pairs, cudaStream_t st);
+int ab_swiglu_bwd(const __nv_bfloat16* dh, const __nv_bfloat16* gu, __nv_bfloat16* dgu, long long pairs,
+                  cudaStream_t st);
 int ab_ce_stats(const __nv_bfloat16* logits, const int64_t* labels, float* stats, int rows, int V,
                 int vocab_start, long long ld, cudaStream_t st);
 int ab_ce_grad(__nv_bfloat16* logits, const int64_t* labels, const float* gstats,

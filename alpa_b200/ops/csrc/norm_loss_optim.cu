@@ -44,11 +44,12 @@ __device__ __forceinline__ float block_max(float v, float* sh) {
 
 // ------------------------------------------------------------------------------------------------
 // LayerNorm.  One CTA per row (grid-stride), 8 bf16 per 128-bit access, row kept in registers.
+// kRms: RMSNorm, the same kernels without the mean and beta: y = x * rstd * g, rstd = rsqrt(mean(x^2) + eps).
 // ------------------------------------------------------------------------------------------------
 constexpr int kLnThreads = 256;
 constexpr int kLnMaxChunks = 8;  // H <= 256 * 8 * 8 = 16384
 
-template <int kChunks>
+template <int kChunks, bool kRms>
 __global__ void __launch_bounds__(kLnThreads)
 layernorm_fwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ res,
                      const __nv_bfloat16* __restrict__ gamma, const __nv_bfloat16* __restrict__ beta,
@@ -92,7 +93,8 @@ layernorm_fwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* _
         for (int j = 0; j < 8; ++j) s += v[c][j];
       }
     }
-    const float mean = block_sum<kLnThreads>(s, sh) / H;
+    float mean = 0.f;
+    if constexpr (!kRms) mean = block_sum<kLnThreads>(s, sh) / H;
     float q = 0.f;
 #pragma unroll
     for (int c = 0; c < kChunks; ++c) {
@@ -116,16 +118,24 @@ layernorm_fwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* _
       const int vi = threadIdx.x + c * kLnThreads;
       if (vi < nvec) {
         int4 g = *reinterpret_cast<const int4*>(gamma + vi * 8);
-        int4 b = *reinterpret_cast<const int4*>(beta + vi * 8);
         const uint32_t* gu = reinterpret_cast<const uint32_t*>(&g);
-        const uint32_t* bu = reinterpret_cast<const uint32_t*>(&b);
         int4 o;
         uint32_t* ou = reinterpret_cast<uint32_t*>(&o);
+        if constexpr (kRms) {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float2 fg = unpack_bf16x2(gu[j]), fb = unpack_bf16x2(bu[j]);
-          ou[j] = pack_bf16x2((v[c][2 * j] - mean) * rstd * fg.x + fb.x,
-                              (v[c][2 * j + 1] - mean) * rstd * fg.y + fb.y);
+          for (int j = 0; j < 4; ++j) {
+            float2 fg = unpack_bf16x2(gu[j]);
+            ou[j] = pack_bf16x2(v[c][2 * j] * rstd * fg.x, v[c][2 * j + 1] * rstd * fg.y);
+          }
+        } else {
+          int4 b = *reinterpret_cast<const int4*>(beta + vi * 8);
+          const uint32_t* bu = reinterpret_cast<const uint32_t*>(&b);
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            float2 fg = unpack_bf16x2(gu[j]), fb = unpack_bf16x2(bu[j]);
+            ou[j] = pack_bf16x2((v[c][2 * j] - mean) * rstd * fg.x + fb.x,
+                                (v[c][2 * j + 1] - mean) * rstd * fg.y + fb.y);
+          }
         }
         *reinterpret_cast<int4*>(y + (size_t)row * H + vi * 8) = o;
       }
@@ -134,7 +144,8 @@ layernorm_fwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* _
 }
 
 // dx = rstd * (g*dy - mean(g*dy) - xhat * mean(g*dy*xhat)) [+ dres];  dgamma += dy*xhat; dbeta += dy
-template <int kChunks>
+// kRms: xhat = x * rstd, no mean(g*dy) term and no dbeta; the per-CTA slots hold dgamma only ([H] instead of [2][H]).
+template <int kChunks, bool kRms>
 __global__ void __launch_bounds__(kLnThreads)
 layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
                      const __nv_bfloat16* __restrict__ gamma, const float* __restrict__ mean,
@@ -148,8 +159,9 @@ layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* 
 #pragma unroll
     for (int j = 0; j < 8; ++j) ag[c][j] = abt[c][j] = 0.f;
 
+  constexpr int kParts = kRms ? 1 : 2;
   for (int row = blockIdx.x; row < rows; row += gridDim.x) {
-    const float mu = mean[row], rs = rstd[row];
+    const float mu = kRms ? 0.f : mean[row], rs = rstd[row];
     float xh[kChunks][8], gd[kChunks][8];
     float s1 = 0.f, s2 = 0.f;
 #pragma unroll
@@ -181,7 +193,8 @@ layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* 
         }
       }
     }
-    const float m1 = block_sum<kLnThreads>(s1, sh) / H;
+    float m1 = 0.f;
+    if constexpr (!kRms) m1 = block_sum<kLnThreads>(s1, sh) / H;
     const float m2 = block_sum<kLnThreads>(s2, sh) / H;
 #pragma unroll
     for (int c = 0; c < kChunks; ++c) {
@@ -215,8 +228,8 @@ layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* 
     if (vi < nvec) {
 #pragma unroll
       for (int j = 0; j < 8; ++j) {  // this CTA's partial sums (reduced in a fixed order by reduce_slots_kernel)
-        ws[(size_t)blockIdx.x * 2 * H + vi * 8 + j] = ag[c][j];
-        ws[(size_t)blockIdx.x * 2 * H + H + vi * 8 + j] = abt[c][j];
+        ws[(size_t)blockIdx.x * kParts * H + vi * 8 + j] = ag[c][j];
+        if constexpr (!kRms) ws[(size_t)blockIdx.x * 2 * H + H + vi * 8 + j] = abt[c][j];
       }
     }
   }
@@ -245,8 +258,9 @@ __device__ __forceinline__ void group_sum2(float& a, float& b, float2 (*xch)[WPR
   }
 }
 
-template <int VPL, int WPR>
-__global__ void __launch_bounds__(256)
+// RMS: two CTAs per SM, else ptxas caps VPL = 8 at 80 registers and spills; 0 (no minimum) keeps LayerNorm's code.
+template <int VPL, int WPR, bool kRms>
+__global__ void __launch_bounds__(256, kRms ? 2 : 0)
 layernorm_fwd_warp_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ res,
                           const __nv_bfloat16* __restrict__ gamma, const __nv_bfloat16* __restrict__ beta,
                           __nv_bfloat16* __restrict__ y, __nv_bfloat16* __restrict__ sum_out,
@@ -280,18 +294,20 @@ layernorm_fwd_warp_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat
         if (sum_out != nullptr) *reinterpret_cast<int4*>(sum_out + (size_t)row * H + off) = v[c];
       }
     }
-    float s = 0.f, dummy = 0.f;
+    float s = 0.f, dummy = 0.f, mean = 0.f;
+    if constexpr (!kRms) {
 #pragma unroll
-    for (int c = 0; c < VPL; ++c) {
-      const uint32_t* a = reinterpret_cast<const uint32_t*>(&v[c]);
+      for (int c = 0; c < VPL; ++c) {
+        const uint32_t* a = reinterpret_cast<const uint32_t*>(&v[c]);
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 f = unpack_bf16x2(a[j]);
-        s += f.x + f.y;
+        for (int j = 0; j < 4; ++j) {
+          const float2 f = unpack_bf16x2(a[j]);
+          s += f.x + f.y;
+        }
       }
+      group_sum2<WPR>(s, dummy, xch, grp, wr, lane, 2 * it);
+      mean = s * (1.f / H);
     }
-    group_sum2<WPR>(s, dummy, xch, grp, wr, lane, 2 * it);
-    const float mean = s * (1.f / H);
     float q = 0.f;
 #pragma unroll
     for (int c = 0; c < VPL; ++c) {
@@ -302,7 +318,9 @@ layernorm_fwd_warp_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat
         q += (f.x - mean) * (f.x - mean) + (f.y - mean) * (f.y - mean);
       }
     }
-    group_sum2<WPR>(q, dummy, xch, grp, wr, lane, 2 * it + 1);
+    // the exchange buffer must alternate between consecutive group sums (a fast warp may start the next one before a
+    // slow warp has read this one's slots): LayerNorm makes two per row, RMSNorm only this one
+    group_sum2<WPR>(q, dummy, xch, grp, wr, lane, kRms ? it : 2 * it + 1);
     const float rstd = rsqrtf(q * (1.f / H) + eps);
     if (lane == 0 && wr == 0) {
       if (mean_out) mean_out[row] = mean;
@@ -312,30 +330,39 @@ layernorm_fwd_warp_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat
     for (int c = 0; c < VPL; ++c) {
       const int off = ((c * WPR + wr) * 32 + lane) * 8;
       const int4 g = *reinterpret_cast<const int4*>(gamma + off);
-      const int4 b = *reinterpret_cast<const int4*>(beta + off);
       const uint32_t* a = reinterpret_cast<const uint32_t*>(&v[c]);
       const uint32_t* gu = reinterpret_cast<const uint32_t*>(&g);
-      const uint32_t* bu = reinterpret_cast<const uint32_t*>(&b);
       int4 o;
       uint32_t* ou = reinterpret_cast<uint32_t*>(&o);
+      if constexpr (kRms) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 f = unpack_bf16x2(a[j]), fg = unpack_bf16x2(gu[j]), fb = unpack_bf16x2(bu[j]);
-        ou[j] = pack_bf16x2((f.x - mean) * rstd * fg.x + fb.x, (f.y - mean) * rstd * fg.y + fb.y);
+        for (int j = 0; j < 4; ++j) {
+          const float2 f = unpack_bf16x2(a[j]), fg = unpack_bf16x2(gu[j]);
+          ou[j] = pack_bf16x2(f.x * rstd * fg.x, f.y * rstd * fg.y);
+        }
+      } else {
+        const int4 b = *reinterpret_cast<const int4*>(beta + off);
+        const uint32_t* bu = reinterpret_cast<const uint32_t*>(&b);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 f = unpack_bf16x2(a[j]), fg = unpack_bf16x2(gu[j]), fb = unpack_bf16x2(bu[j]);
+          ou[j] = pack_bf16x2((f.x - mean) * rstd * fg.x + fb.x, (f.y - mean) * rstd * fg.y + fb.y);
+        }
       }
       *reinterpret_cast<int4*>(y + (size_t)row * H + off) = o;
     }
   }
 }
 
-template <int VPL, int WPR>
+template <int VPL, int WPR, bool kRms>
 __global__ void __launch_bounds__(256)
 layernorm_bwd_warp_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
                           const __nv_bfloat16* __restrict__ gamma, const float* __restrict__ mean,
                           const float* __restrict__ rstd, const __nv_bfloat16* __restrict__ dres,
                           __nv_bfloat16* __restrict__ dx, float* __restrict__ ws, int rows) {
   constexpr int H = VPL * WPR * 256;
-  extern __shared__ float sh_gb[];   // [row groups][2][H]
+  constexpr int kParts = kRms ? 1 : 2;
+  extern __shared__ float sh_gb[];   // [row groups][kParts][H]
   __shared__ float2 xch[16][WPR];
   const int lane = threadIdx.x & 31;
   const int wib = threadIdx.x >> 5;
@@ -349,7 +376,7 @@ layernorm_bwd_warp_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloa
     for (int j = 0; j < 8; ++j) ag[c][j] = ab[c][j] = 0.f;
   int it = 0;
   for (int row = blockIdx.x * groups_per_cta + grp; row < rows; row += ngroups, ++it) {
-    const float mu = mean[row], rs = rstd[row];
+    const float mu = kRms ? 0.f : mean[row], rs = rstd[row];
     int4 xv[VPL], dv[VPL];
 #pragma unroll
     for (int c = 0; c < VPL; ++c) {
@@ -378,7 +405,7 @@ layernorm_bwd_warp_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloa
       }
     }
     group_sum2<WPR>(s1, s2, xch, grp, wr, lane, it);
-    const float m1 = s1 * (1.f / H), m2 = s2 * (1.f / H);
+    const float m1 = kRms ? 0.f : s1 * (1.f / H), m2 = s2 * (1.f / H);
 #pragma unroll
     for (int c = 0; c < VPL; ++c) {
       const int off = ((c * WPR + wr) * 32 + lane) * 8;
@@ -408,14 +435,14 @@ layernorm_bwd_warp_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloa
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const int col = ((c * WPR + wr) * 32 + lane) * 8 + j;
-      sh_gb[grp * 2 * H + col] = ag[c][j];
-      sh_gb[grp * 2 * H + H + col] = ab[c][j];
+      sh_gb[grp * kParts * H + col] = ag[c][j];
+      if constexpr (!kRms) sh_gb[grp * 2 * H + H + col] = ab[c][j];
     }
   __syncthreads();
-  for (int i = threadIdx.x; i < 2 * H; i += blockDim.x) {
+  for (int i = threadIdx.x; i < kParts * H; i += blockDim.x) {
     float t = 0.f;
-    for (int g = 0; g < groups_per_cta; ++g) t += sh_gb[g * 2 * H + i];
-    ws[(size_t)blockIdx.x * 2 * H + i] = t;
+    for (int g = 0; g < groups_per_cta; ++g) t += sh_gb[g * kParts * H + i];
+    ws[(size_t)blockIdx.x * kParts * H + i] = t;
   }
 }
 
@@ -714,14 +741,14 @@ sumsq_kernel(const AdamTensor* __restrict__ tensors, const AdamChunk* __restrict
 
 using namespace ab;
 
-template <int kChunks>
+template <int kChunks, bool kRms>
 static void ln_fwd_launch(const LayerNormArgs& a, cudaStream_t st, int grid) {
-  layernorm_fwd_kernel<kChunks><<<grid, kLnThreads, 0, st>>>(
+  layernorm_fwd_kernel<kChunks, kRms><<<grid, kLnThreads, 0, st>>>(
       a.x, a.residual, a.gamma, a.beta, a.y, a.sum_out, a.mean, a.rstd, a.rows, a.H, a.eps);
 }
-template <int kChunks>
+template <int kChunks, bool kRms>
 static void ln_bwd_launch(const LayerNormBwdArgs& a, cudaStream_t st, int grid) {
-  layernorm_bwd_kernel<kChunks><<<grid, kLnThreads, 0, st>>>(
+  layernorm_bwd_kernel<kChunks, kRms><<<grid, kLnThreads, 0, st>>>(
       a.dy, a.x, a.gamma, a.mean, a.rstd, a.dres, a.dx, a.ws, a.rows, a.H);
 }
 static int ln_bwd_generic_grid(int rows) { return rows < ab::num_sms() * 2 ? rows : ab::num_sms() * 2; }
@@ -736,7 +763,7 @@ static int ln_bwd_warp_grid(int rows) {
   return grid;
 }
 
-template <int VPL, int WPR>
+template <int VPL, int WPR, bool kRms>
 static void ln_fwd_warp_launch(const LayerNormArgs& a, cudaStream_t st) {
   const int gpc = 8 / WPR;
   int grid = (a.rows + gpc - 1) / gpc;
@@ -746,52 +773,55 @@ static void ln_fwd_warp_launch(const LayerNormArgs& a, cudaStream_t st) {
     const int iters = (a.rows + ab::num_sms() * 8 * gpc - 1) / (ab::num_sms() * 8 * gpc);
     grid = (a.rows + iters * gpc - 1) / (iters * gpc);
   }
-  layernorm_fwd_warp_kernel<VPL, WPR><<<grid, 256, 0, st>>>(a.x, a.residual, a.gamma, a.beta, a.y, a.sum_out,
-                                                            a.mean, a.rstd, a.rows, a.eps);
+  layernorm_fwd_warp_kernel<VPL, WPR, kRms><<<grid, 256, 0, st>>>(a.x, a.residual, a.gamma, a.beta, a.y, a.sum_out,
+                                                                  a.mean, a.rstd, a.rows, a.eps);
 }
-template <int VPL, int WPR>
+template <int VPL, int WPR, bool kRms>
 static void ln_bwd_warp_launch(const LayerNormBwdArgs& a, cudaStream_t st) {
   const int gpc = 8 / WPR;
   constexpr int H = VPL * WPR * 256;
   const int grid = ln_bwd_warp_grid<WPR>(a.rows);
-  const int smem = gpc * 2 * H * (int)sizeof(float);
+  const int smem = gpc * (kRms ? 1 : 2) * H * (int)sizeof(float);
   static bool attr_set = false;
   if (!attr_set) {
-    cudaFuncSetAttribute(layernorm_bwd_warp_kernel<VPL, WPR>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaFuncSetAttribute(layernorm_bwd_warp_kernel<VPL, WPR, kRms>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     attr_set = true;
   }
-  layernorm_bwd_warp_kernel<VPL, WPR><<<grid, 256, smem, st>>>(
+  layernorm_bwd_warp_kernel<VPL, WPR, kRms><<<grid, 256, smem, st>>>(
       a.dy, a.x, a.gamma, a.mean, a.rstd, a.dres, a.dx, a.ws, a.rows);
 }
 
-extern "C" int ab_layernorm_fwd(const LayerNormArgs* a, cudaStream_t st) {
-  if (a->H % 8 != 0 || a->H > kLnThreads * 8 * kLnMaxChunks) return 1;
+template <bool kRms>
+static void ln_fwd_dispatch(const LayerNormArgs* a, cudaStream_t st) {
   if (a->H % 256 == 0 && a->H <= 8192) {
     switch (a->H / 256) {
-      case 1: ln_fwd_warp_launch<1, 1>(*a, st); break;
-      case 2: ln_fwd_warp_launch<2, 1>(*a, st); break;
-      case 3: ln_fwd_warp_launch<3, 1>(*a, st); break;
-      case 4: ln_fwd_warp_launch<4, 1>(*a, st); break;
-      case 6: ln_fwd_warp_launch<6, 1>(*a, st); break;
-      case 8: ln_fwd_warp_launch<8, 1>(*a, st); break;
-      case 10: ln_fwd_warp_launch<5, 2>(*a, st); break;
-      case 12: ln_fwd_warp_launch<6, 2>(*a, st); break;
-      case 16: ln_fwd_warp_launch<8, 2>(*a, st); break;
-      case 20: ln_fwd_warp_launch<5, 4>(*a, st); break;
-      case 24: ln_fwd_warp_launch<6, 4>(*a, st); break;
-      case 28: ln_fwd_warp_launch<7, 4>(*a, st); break;
-      case 32: ln_fwd_warp_launch<8, 4>(*a, st); break;
-      default: goto generic_fwd;
+      case 1: ln_fwd_warp_launch<1, 1, kRms>(*a, st); return;
+      case 2: ln_fwd_warp_launch<2, 1, kRms>(*a, st); return;
+      case 3: ln_fwd_warp_launch<3, 1, kRms>(*a, st); return;
+      case 4: ln_fwd_warp_launch<4, 1, kRms>(*a, st); return;
+      case 6: ln_fwd_warp_launch<6, 1, kRms>(*a, st); return;
+      case 8: ln_fwd_warp_launch<8, 1, kRms>(*a, st); return;
+      case 10: ln_fwd_warp_launch<5, 2, kRms>(*a, st); return;
+      case 12: ln_fwd_warp_launch<6, 2, kRms>(*a, st); return;
+      case 16: ln_fwd_warp_launch<8, 2, kRms>(*a, st); return;
+      case 20: ln_fwd_warp_launch<5, 4, kRms>(*a, st); return;
+      case 24: ln_fwd_warp_launch<6, 4, kRms>(*a, st); return;
+      case 28: ln_fwd_warp_launch<7, 4, kRms>(*a, st); return;
+      case 32: ln_fwd_warp_launch<8, 4, kRms>(*a, st); return;
+      default: break;
     }
-    return cudaGetLastError() == cudaSuccess ? 0 : 2;
   }
-generic_fwd:
   const int chunks = (a->H / 8 + kLnThreads - 1) / kLnThreads;
   const int grid = a->rows < ab::num_sms() * 8 ? a->rows : ab::num_sms() * 8;
-  if (chunks <= 1) ln_fwd_launch<1>(*a, st, grid);
-  else if (chunks <= 2) ln_fwd_launch<2>(*a, st, grid);
-  else if (chunks <= 4) ln_fwd_launch<4>(*a, st, grid);
-  else ln_fwd_launch<8>(*a, st, grid);
+  if (chunks <= 1) ln_fwd_launch<1, kRms>(*a, st, grid);
+  else if (chunks <= 2) ln_fwd_launch<2, kRms>(*a, st, grid);
+  else if (chunks <= 4) ln_fwd_launch<4, kRms>(*a, st, grid);
+  else ln_fwd_launch<8, kRms>(*a, st, grid);
+}
+extern "C" int ab_layernorm_fwd(const LayerNormArgs* a, cudaStream_t st) {
+  if (a->H % 8 != 0 || a->H > kLnThreads * 8 * kLnMaxChunks) return 1;
+  if (a->rms) ln_fwd_dispatch<true>(a, st);
+  else ln_fwd_dispatch<false>(a, st);
   return cudaGetLastError() == cudaSuccess ? 0 : 2;
 }
 // (VPL, WPR) of the warp-group kernel for H, or 0 when the generic kernel runs
@@ -803,7 +833,7 @@ static int ln_bwd_warp_cfg(int H) {
   }
   return 0;
 }
-// Number of per-CTA partial rows ([2][H] floats each) ab_layernorm_bwd writes into a.ws.
+// Number of per-CTA partial rows ([2][H] floats each, [H] for RMSNorm) ab_layernorm_bwd writes into a.ws.
 extern "C" int ab_layernorm_bwd_slots(int rows, int H) {
   const int cfg = ln_bwd_warp_cfg(H);
   if (cfg == 0) return ln_bwd_generic_grid(rows);
@@ -814,33 +844,39 @@ extern "C" int ab_layernorm_bwd_slots(int rows, int H) {
     default: return ln_bwd_warp_grid<8>(rows);
   }
 }
-extern "C" int ab_layernorm_bwd(const LayerNormBwdArgs* a, cudaStream_t st) {
-  if (a->H % 8 != 0 || a->H > kLnThreads * 8 * 4 || a->ws == nullptr) return 1;
+template <bool kRms>
+static void ln_bwd_dispatch(const LayerNormBwdArgs* a, cudaStream_t st) {
   switch (ln_bwd_warp_cfg(a->H)) {
-    case 11: ln_bwd_warp_launch<1, 1>(*a, st); break;
-    case 21: ln_bwd_warp_launch<2, 1>(*a, st); break;
-    case 31: ln_bwd_warp_launch<3, 1>(*a, st); break;
-    case 41: ln_bwd_warp_launch<4, 1>(*a, st); break;
-    case 32: ln_bwd_warp_launch<3, 2>(*a, st); break;
-    case 42: ln_bwd_warp_launch<4, 2>(*a, st); break;
-    case 52: ln_bwd_warp_launch<5, 2>(*a, st); break;
-    case 34: ln_bwd_warp_launch<3, 4>(*a, st); break;
-    case 44: ln_bwd_warp_launch<4, 4>(*a, st); break;
-    case 54: ln_bwd_warp_launch<5, 4>(*a, st); break;
-    case 38: ln_bwd_warp_launch<3, 8>(*a, st); break;
-    case 48: ln_bwd_warp_launch<4, 8>(*a, st); break;
+    case 11: ln_bwd_warp_launch<1, 1, kRms>(*a, st); break;
+    case 21: ln_bwd_warp_launch<2, 1, kRms>(*a, st); break;
+    case 31: ln_bwd_warp_launch<3, 1, kRms>(*a, st); break;
+    case 41: ln_bwd_warp_launch<4, 1, kRms>(*a, st); break;
+    case 32: ln_bwd_warp_launch<3, 2, kRms>(*a, st); break;
+    case 42: ln_bwd_warp_launch<4, 2, kRms>(*a, st); break;
+    case 52: ln_bwd_warp_launch<5, 2, kRms>(*a, st); break;
+    case 34: ln_bwd_warp_launch<3, 4, kRms>(*a, st); break;
+    case 44: ln_bwd_warp_launch<4, 4, kRms>(*a, st); break;
+    case 54: ln_bwd_warp_launch<5, 4, kRms>(*a, st); break;
+    case 38: ln_bwd_warp_launch<3, 8, kRms>(*a, st); break;
+    case 48: ln_bwd_warp_launch<4, 8, kRms>(*a, st); break;
     default: {
       const int chunks = (a->H / 8 + kLnThreads - 1) / kLnThreads;
       const int grid = ln_bwd_generic_grid(a->rows);
-      if (chunks <= 1) ln_bwd_launch<1>(*a, st, grid);
-      else if (chunks <= 2) ln_bwd_launch<2>(*a, st, grid);
-      else ln_bwd_launch<4>(*a, st, grid);
+      if (chunks <= 1) ln_bwd_launch<1, kRms>(*a, st, grid);
+      else if (chunks <= 2) ln_bwd_launch<2, kRms>(*a, st, grid);
+      else ln_bwd_launch<4, kRms>(*a, st, grid);
     }
   }
+}
+extern "C" int ab_layernorm_bwd(const LayerNormBwdArgs* a, cudaStream_t st) {
+  if (a->H % 8 != 0 || a->H > kLnThreads * 8 * 4 || a->ws == nullptr) return 1;
+  if (a->rms) ln_bwd_dispatch<true>(a, st);
+  else ln_bwd_dispatch<false>(a, st);
   const int slots = ab_layernorm_bwd_slots(a->rows, a->H);
   const int blocks = (a->H + 255) / 256;
-  reduce_slots_kernel<<<blocks, 256, 0, st>>>(a->ws, slots, 2LL * a->H, a->H, a->dgamma);
-  reduce_slots_kernel<<<blocks, 256, 0, st>>>(a->ws + a->H, slots, 2LL * a->H, a->H, a->dbeta);
+  const long long ld = (a->rms ? 1LL : 2LL) * a->H;
+  reduce_slots_kernel<<<blocks, 256, 0, st>>>(a->ws, slots, ld, a->H, a->dgamma);
+  if (!a->rms) reduce_slots_kernel<<<blocks, 256, 0, st>>>(a->ws + a->H, slots, ld, a->H, a->dbeta);
   return cudaGetLastError() == cudaSuccess ? 0 : 2;
 }
 extern "C" int ab_ce_stats(const __nv_bfloat16* logits, const int64_t* labels, float* stats, int rows,

@@ -18,7 +18,8 @@ from alpa_b200.global_env import global_config
 
 __all__ = [
     "linear", "linear_act", "linear_dgrad", "linear_dgrad_add", "linear_wgrad", "bias_grad", "act_bwd", "layer_norm",
-    "add_layer_norm", "layer_norm_bwd", "attention", "attention_bwd", "attention_gqa_packed",
+    "add_layer_norm", "layer_norm_bwd", "rms_norm", "add_rms_norm", "rms_norm_bwd", "rotary_packed", "swiglu",
+    "swiglu_bwd", "attention", "attention_bwd", "attention_gqa_packed",
     "attention_gqa_packed_bwd", "embedding", "embedding_bwd",
     "cross_entropy", "cross_entropy_bwd", "fused_adamw_", "pipeline_marker",
     "bmm", "moe_dispatch", "moe_combine", "moe_combine_wgrad", "moe_top2_route", "linear_fp8", "linear_decode", "decode_attention", "ragged_attention",
@@ -401,6 +402,102 @@ def _aln_bwd(ctx, dy, ds, dmean, drstd):
 add_layer_norm.register_autograd(_aln_bwd, setup_context=_aln_setup)
 
 
+# ---- RMSNorm: the LayerNorm kernels' `rms` variant (no mean, no beta): y = x * rstd * g, rstd = rsqrt(mean(x^2) + eps)
+def _rms_ref(x: Tensor, g: Tensor, eps: float):
+    xf = x.float()
+    rstd = torch.rsqrt(xf.pow(2).mean(-1) + eps)
+    return (xf * rstd[..., None] * g.float()).to(x.dtype), rstd
+
+
+@torch.library.custom_op("alpa_b200::rms_norm", mutates_args=())
+def rms_norm(x: Tensor, g: Tensor, eps: float) -> Tuple[Tensor, Tensor]:
+    """(y, rstd); rstd is fp32 with shape x.shape[:-1]."""
+    if C := _kernels("rms_norm", x, g, unsupported=_ln_unsupported(x.shape[-1])):
+        y, _, rstd, _ = C.layernorm_fwd(x.contiguous(), None, g, None, eps, False, rms=True)
+        return y, rstd.view(x.shape[:-1])
+    return _rms_ref(x, g, eps)
+
+
+@rms_norm.register_fake
+def _(x, g, eps):
+    return torch.empty_like(x), x.new_empty(x.shape[:-1], dtype=torch.float32)
+
+
+@torch.library.custom_op("alpa_b200::add_rms_norm", mutates_args=())
+def add_rms_norm(x: Tensor, r: Tensor, g: Tensor, eps: float) -> Tuple[Tensor, Tensor, Tensor]:
+    """s = x + r (rounded to x's dtype); (rms_norm(s), s, rstd) in one pass."""
+    if C := _kernels("add_rms_norm", x, r, g, unsupported=_ln_unsupported(x.shape[-1])):
+        y, _, rstd, s = C.layernorm_fwd(x.contiguous(), r.contiguous(), g, None, eps, True, rms=True)
+        return y, s, rstd.view(x.shape[:-1])
+    s = x + r
+    y, rstd = _rms_ref(s, g, eps)
+    return y, s, rstd
+
+
+@add_rms_norm.register_fake
+def _(x, r, g, eps):
+    return torch.empty_like(x), torch.empty_like(x), x.new_empty(x.shape[:-1], dtype=torch.float32)
+
+
+@torch.library.custom_op("alpa_b200::rms_norm_bwd", mutates_args=())
+def rms_norm_bwd(dy: Tensor, x: Tensor, g: Tensor, rstd: Tensor, dres: Optional[Tensor]) -> Tuple[Tensor, Tensor]:
+    """(dx [+ dres], dgamma) of y = rms_norm(x): dx = rstd * (g*dy - xhat * mean(g*dy*xhat)), xhat = x * rstd."""
+    H = x.shape[-1]
+    if C := _kernels("rms_norm_bwd", dy, x, g, unsupported=_ln_unsupported(H)):
+        dg = torch.zeros(H, device=x.device, dtype=torch.float32)
+        dx = C.layernorm_bwd(dy.contiguous(), x.contiguous(), g, None, rstd.reshape(-1).contiguous(),
+                             dres.contiguous() if dres is not None else None, dg, None, rms=True)
+        return dx, dg.to(g.dtype)
+    xf, df = x.float(), dy.float()
+    xh = xf * rstd[..., None]
+    gd = df * g.float()
+    dx = rstd[..., None] * (gd - xh * (gd * xh).mean(-1, keepdim=True))
+    if dres is not None:
+        dx = dx + dres.float()
+    dg = (df * xh).reshape(-1, H).sum(0)
+    return dx.to(x.dtype), dg.to(g.dtype)
+
+
+@rms_norm_bwd.register_fake
+def _(dy, x, g, rstd, dres):
+    return torch.empty_like(x), torch.empty_like(g)
+
+
+def _rms_setup(ctx, inputs, output):
+    ctx.set_materialize_grads(False)  # unused outputs yield None, not a zero tensor + add
+    x, g, eps = inputs
+    ctx.save_for_backward(x, g, output[1])
+
+
+def _rms_bwd(ctx, dy, drstd):
+    if dy is None:
+        return None, None, None
+    x, g, rstd = ctx.saved_tensors
+    dx, dg = rms_norm_bwd(dy, x, g, rstd, None)
+    return dx, dg, None
+
+
+rms_norm.register_autograd(_rms_bwd, setup_context=_rms_setup)
+
+
+def _arms_setup(ctx, inputs, output):
+    ctx.set_materialize_grads(False)  # unused outputs yield None, not a zero tensor + add
+    x, r, g, eps = inputs
+    _, s, rstd = output
+    ctx.save_for_backward(s, g, rstd)
+
+
+def _arms_bwd(ctx, dy, ds, drstd):
+    s, g, rstd = ctx.saved_tensors
+    if dy is None:
+        return ds, ds, None, None
+    dx, dg = rms_norm_bwd(dy, s, g, rstd, ds)
+    return dx, dx, dg, None
+
+
+add_rms_norm.register_autograd(_arms_bwd, setup_context=_arms_setup)
+
+
 # =================================================================================================
 # attention: q, k, v are [B, S, heads, D]
 # =================================================================================================
@@ -588,6 +685,122 @@ def _attn_gqa_bwd(ctx, do, dlse):
 
 
 attention_gqa_packed.register_autograd(_attn_gqa_bwd, setup_context=_attn_packed_setup)
+
+
+# ---- rotary position embedding on the packed [B, S, Hkv, G + 2, D] tensor (HF's rotate_half convention): slots 0..G
+# (the query heads and K) rotate, slot G + 1 (V) passes through.  Element i pairs with i + D/2 at angle
+# float(position) * inv_freq[i], inv_freq = 1 / theta ** (arange(0, D, 2) / D) as HF builds it.
+@cache
+def _inv_freq(D: int, theta: float, device: str) -> Tensor:
+    """HF's default rope frequencies, computed on the CPU as HF does and cached per (D, theta, device)."""
+    return (1.0 / (theta ** (torch.arange(0, D, 2, dtype=torch.int64).float() / D))).to(device)
+
+
+def _rotary_ref(qkv: Tensor, position_ids: Tensor, inv_freq: Tensor, inverse: bool) -> Tensor:
+    D, R = qkv.shape[-1], qkv.shape[3] - 1
+    ang = position_ids.float()[..., None] * inv_freq                  # [B, S, D/2], the fp32 product HF forms
+    c, s = ang.cos()[:, :, None, None], ang.sin()[:, :, None, None]
+    if inverse:
+        s = -s
+    x = qkv[:, :, :, :R].float()
+    x1, x2 = x[..., :D // 2], x[..., D // 2:]
+    rot = torch.cat([x1 * c - x2 * s, x2 * c + x1 * s], -1).to(qkv.dtype)
+    return torch.cat([rot, qkv[:, :, :, R:]], 3)
+
+
+def _rotary_unsupported(qkv: Tensor) -> Optional[str]:
+    """Why the rotary kernel (8 elements of each half per vector) cannot take qkv, or None."""
+    if qkv.shape[-1] % 16:
+        return "head dim not a multiple of 16"
+    return None if qkv.is_contiguous() and qkv.data_ptr() % 16 == 0 else "packed qkv not contiguous"
+
+
+@torch.library.custom_op("alpa_b200::rotary_packed", mutates_args=())
+def rotary_packed(qkv: Tensor, position_ids: Tensor, theta: float, inverse: bool) -> Tensor:
+    """qkv [B,S,Hkv,G+2,D] with the G query heads and K of every K/V head rotated by position_ids (by minus the angle
+    when `inverse`, which is the backward); V copied.  position_ids: integer, [B, S] or broadcastable to it (HF's
+    [1, S]), on qkv's device."""
+    inv_freq = _inv_freq(qkv.shape[-1], float(theta), str(qkv.device))
+    if C := _kernels("rotary_packed", qkv, position_ids, unsupported=lambda: _rotary_unsupported(qkv)):
+        pos = position_ids.to(torch.int64).expand(qkv.shape[0], qkv.shape[1]).contiguous()
+        return C.rotary_packed(qkv, pos, inv_freq, inverse)
+    return _rotary_ref(qkv, position_ids, inv_freq, inverse)
+
+
+@rotary_packed.register_fake
+def _(qkv, position_ids, theta, inverse):
+    return torch.empty_like(qkv)
+
+
+def _rotary_setup(ctx, inputs, output):
+    ctx.set_materialize_grads(False)  # unused outputs yield None, not a zero tensor + add
+    _, position_ids, theta, inverse = inputs
+    ctx.save_for_backward(position_ids)
+    ctx.theta, ctx.inverse = theta, inverse
+
+
+def _rotary_bwd(ctx, dy):
+    if dy is None:
+        return None, None, None, None
+    (position_ids,) = ctx.saved_tensors
+    return rotary_packed(dy, position_ids, ctx.theta, not ctx.inverse), None, None, None
+
+
+rotary_packed.register_autograd(_rotary_bwd, setup_context=_rotary_setup)
+
+
+# ---- SwiGLU on interleaved pairs: gu [..., I, 2] holds (gate j, up j) at fc1 output features (2j, 2j + 1), so a
+# contiguous column split of fc1 keeps every pair on one device.
+def _swiglu_unsupported(*ts: Tensor) -> Optional[str]:
+    """Why the SwiGLU kernels (4 pairs per 16-byte vector) cannot take these operands, or None."""
+    if ts[-1].shape[-2] % 4:
+        return "I not a multiple of 4"
+    return None if all(t.is_contiguous() and t.data_ptr() % 16 == 0 for t in ts) else "operands not contiguous"
+
+
+@torch.library.custom_op("alpa_b200::swiglu", mutates_args=())
+def swiglu(gu: Tensor) -> Tensor:
+    """h [..., I] = silu(gu[..., 0]) * gu[..., 1]"""
+    if C := _kernels("swiglu", gu, unsupported=lambda: _swiglu_unsupported(gu)):
+        return C.swiglu_fwd(gu)
+    g, u = gu.float().unbind(-1)
+    return (F.silu(g) * u).to(gu.dtype)
+
+
+@swiglu.register_fake
+def _(gu):
+    return gu.new_empty(gu.shape[:-1])
+
+
+@torch.library.custom_op("alpa_b200::swiglu_bwd", mutates_args=())
+def swiglu_bwd(dh: Tensor, gu: Tensor) -> Tensor:
+    """dgu [..., I, 2] = (dh * u * s (1 + g (1 - s)), dh * silu(g)), s = sigmoid(g): recomputed from gu."""
+    if C := _kernels("swiglu_bwd", dh, gu, unsupported=lambda: _swiglu_unsupported(dh[..., None], gu)):
+        return C.swiglu_bwd(dh, gu)
+    g, u = gu.float().unbind(-1)
+    d = dh.float()
+    s = torch.sigmoid(g)
+    return torch.stack([d * u * s * (1 + g * (1 - s)), d * g * s], -1).to(gu.dtype)
+
+
+@swiglu_bwd.register_fake
+def _(dh, gu):
+    return torch.empty_like(gu)
+
+
+def _swiglu_setup(ctx, inputs, output):
+    ctx.set_materialize_grads(False)  # unused outputs yield None, not a zero tensor + add
+    ctx.save_for_backward(inputs[0])
+
+
+def _swiglu_grad(ctx, dh):
+    if dh is None:
+        return None
+    (gu,) = ctx.saved_tensors
+    return swiglu_bwd(dh, gu)
+
+
+swiglu.register_autograd(_swiglu_grad, setup_context=_swiglu_setup)
 
 # =================================================================================================
 # embedding (token gather [+ position]) -- the reference lowers this to a one-hot matmul

@@ -680,8 +680,9 @@ def rule_ab_bias_grad(node: fx.Node) -> OpSig:
 
 
 def rule_ab_layer_norm(node: fx.Node) -> OpSig:
-    """layer_norm(x,g,b,eps) / add_layer_norm(x,r,g,b,eps)"""
-    is_add = node.target == torch.ops.alpa_b200.add_layer_norm.default
+    """layer_norm(x,g,b,eps) / add_layer_norm(x,r,g,b,eps) and their RMS forms rms_norm(x,g,eps) /
+    add_rms_norm(x,r,g,eps): rows shard, the normalised dim never does"""
+    is_add = node.target in (torch.ops.alpa_b200.add_layer_norm.default, torch.ops.alpa_b200.add_rms_norm.default)
     x = node.args[0]
     sig = OpSig()
     xs = _shape(x)
@@ -703,18 +704,24 @@ def rule_ab_layer_norm(node: fx.Node) -> OpSig:
 
 
 def rule_ab_layer_norm_bwd(node: fx.Node) -> OpSig:
-    dy, x, g, mean, rstd, dres = node.args[:6]
+    """layer_norm_bwd(dy,x,g,mean,rstd,dres) -> (dx,dgamma,dbeta) / rms_norm_bwd(dy,x,g,rstd,dres) -> (dx,dgamma)"""
+    if node.target == torch.ops.alpa_b200.rms_norm_bwd.default:
+        dy, x, g, rstd, dres = node.args[:5]
+        stats = [rstd]
+    else:
+        dy, x, g, mean, rstd, dres = node.args[:6]
+        stats = [mean, rstd]
     sig = OpSig()
     xs = _shape(x)
     lead = _lead_labels(sig, xs[:-1])
     lh = sig.new(xs[-1], NOSHARD)
-    sig.operands += [(dy, lead + [lh]), (x, lead + [lh]), (g, [lh]), (mean, list(lead)), (rstd, list(lead))]
+    sig.operands += [(dy, lead + [lh]), (x, lead + [lh]), (g, [lh])] + [(t, list(lead)) for t in stats]
     if _is_tensor_node(dres):
         sig.operands.append((dres, lead + [lh]))
     v = _val(node)
     sig.outputs.append((tuple(int(s) for s in v[0].shape), lead + [lh], v[0].dtype))
-    sig.outputs.append((tuple(int(s) for s in v[1].shape), [lh], v[1].dtype))   # dgamma: partial over rows
-    sig.outputs.append((tuple(int(s) for s in v[2].shape), [lh], v[2].dtype))
+    for t in v[1:]:   # dgamma (and dbeta): partial over rows
+        sig.outputs.append((tuple(int(s) for s in t.shape), [lh], t.dtype))
     sig.follow = 0
     return sig
 
@@ -798,6 +805,42 @@ def rule_ab_attention_gqa_packed(node: fx.Node) -> OpSig:
         sig.outputs.append((tuple(int(s) for s in vals[1].shape), list(stat), vals[1].dtype))
         sig.follow = 0
         sig.flops = 4.0 * B * Hkv * G * S_ * S_ * D
+    return sig
+
+
+def rule_ab_rotary_packed(node: fx.Node) -> OpSig:
+    """rotary_packed(qkv[B,S,Hkv,G+2,D], position_ids[B,S], theta, inverse): batch and K/V heads shard; the slot dim and
+    D (whose halves pair up) never do, and position_ids shares the batch and sequence labels (none on a broadcast
+    batch dim: HF's [1, S])."""
+    qkv, pos = node.args[:2]
+    sig = OpSig()
+    B, S_, Hkv, P, D = _shape(qkv)
+    lb, ls, lkv = sig.new(B), sig.new(S_, NOSHARD), sig.new(Hkv)
+    labels = [lb, ls, lkv, sig.new(P, NOSHARD), sig.new(D, NOSHARD)]
+    pos_b = _shape(pos)[0]
+    sig.operands += [(qkv, labels), (pos, [lb if pos_b == B else -1, ls])]
+    t = _out_vals(node)[0]
+    sig.outputs.append((tuple(int(s) for s in t.shape), list(labels), t.dtype))
+    sig.follow = 0
+    return sig
+
+
+def rule_ab_swiglu(node: fx.Node) -> OpSig:
+    """swiglu(gu[...,I,2]) -> h[...,I] / swiglu_bwd(dh[...,I], gu) -> dgu: the leading dims and I shard, the
+    (gate, up) pair dim never does."""
+    is_bwd = node.target == torch.ops.alpa_b200.swiglu_bwd.default
+    gu = node.args[1] if is_bwd else node.args[0]
+    sig = OpSig()
+    gs = _shape(gu)
+    lead = _lead_labels(sig, gs[:-1])
+    pair = lead + [sig.new(gs[-1], NOSHARD)]
+    if is_bwd:
+        sig.operands += [(node.args[0], list(lead)), (gu, pair)]
+    else:
+        sig.operands.append((gu, pair))
+    t = _out_vals(node)[0]
+    sig.outputs.append((tuple(int(s) for s in t.shape), pair if is_bwd else list(lead), t.dtype))
+    sig.follow = 1 if is_bwd else 0
     return sig
 
 
@@ -1141,8 +1184,11 @@ _SDPA_OPS = [getattr(aten, n).default for n in (
     "_scaled_dot_product_flash_attention", "_scaled_dot_product_flash_attention_backward",
     "_scaled_dot_product_cudnn_attention", "_scaled_dot_product_cudnn_attention_backward") if hasattr(aten, n)]
 _reg(_SDPA_OPS, rule_sdpa)
-_reg([_ab.layer_norm.default, _ab.add_layer_norm.default], rule_ab_layer_norm)
-_reg([_ab.layer_norm_bwd.default], rule_ab_layer_norm_bwd)
+_reg([_ab.layer_norm.default, _ab.add_layer_norm.default, _ab.rms_norm.default, _ab.add_rms_norm.default],
+     rule_ab_layer_norm)
+_reg([_ab.layer_norm_bwd.default, _ab.rms_norm_bwd.default], rule_ab_layer_norm_bwd)
+_reg([_ab.rotary_packed.default], rule_ab_rotary_packed)
+_reg([_ab.swiglu.default, _ab.swiglu_bwd.default], rule_ab_swiglu)
 _reg([_ab.attention.default], rule_ab_attention)
 _reg([_ab.attention_bwd.default], rule_ab_attention_bwd)
 _reg([_ab.attention_cached.default], rule_ab_attention_cached)

@@ -2,7 +2,7 @@
 calls after 5 warm-ups).  The kernels' numerics are checked by the GPU tests under tests/.
 
 usage: python scripts/gpu_check.py [section ...]
-  sections: gemm_bench gemm_sweep misc attn attn_gqa moe fp8 gemv ragged (default: all)
+  sections: gemm_bench gemm_sweep misc attn attn_gqa moe fp8 gemv ragged llama llama_step (default: all)
 gemm_bench also checks the outputs it times; the exit code is non-zero if one is wrong.
 """
 import math
@@ -294,8 +294,143 @@ def sec_ragged():
         print(f"BENCH ragged_attention h{h} D{D} T{T}: {t * 1e3:.1f} us, {kv_bytes / t / 1e6:.0f} GB/s of K/V streamed")
 
 
+# The 1.3B-sized Llama-style config of the llama sections: 16 x 1024 tokens, H = 2048, 32 query heads, 8 K/V heads,
+# D = 64, I = 5504 (GPT-1.3B's width and depth with Llama's block).
+LLAMA_B, LLAMA_S, LLAMA_H, LLAMA_HQ, LLAMA_HKV, LLAMA_I = 16, 1024, 2048, 32, 8, 5504
+
+
+def sec_llama():
+    """RMSNorm, rotary and SwiGLU at the Llama-style step shapes, L2 flushed, against the LayerNorm kernel and the eager
+    PyTorch compositions a user would otherwise run (F.rms_norm; HF's cos / sin and apply_rotary_pos_emb on separate
+    q / k; F.silu(g) * u on the interleaved pairs).  GB/s counts the bytes each op must move at least."""
+    from transformers.models.llama.modeling_llama import apply_rotary_pos_emb
+    F = torch.nn.functional
+    bf = torch.bfloat16
+    T, H, Hq, Hkv, I = LLAMA_B * LLAMA_S, LLAMA_H, LLAMA_HQ, LLAMA_HKV, LLAMA_I
+    D, G = H // Hq, Hq // Hkv
+
+    def row(name, t, nbytes):
+        print(f"BENCH llama {name}: {t * 1e3:.1f} us  {nbytes / t / 1e6:.0f} GB/s", flush=True)
+
+    x = torch.randn(T, H, device=dev, dtype=bf)
+    g = (1 + 0.1 * torch.randn(H, device=dev)).to(bf)
+    b = torch.zeros(H, device=dev, dtype=bf)
+    dy = torch.randn(T, H, device=dev, dtype=bf)
+    row(f"rmsnorm fwd {T}x{H}", median_ms(lambda: _C.layernorm_fwd(x, None, g, None, 1e-5, False, rms=True),
+                                          flush=True), 2 * T * H * 2)
+    row(f"layernorm fwd {T}x{H}", median_ms(lambda: _C.layernorm_fwd(x, None, g, b, 1e-5, False), flush=True),
+        2 * T * H * 2)
+    row(f"F.rms_norm(lib) fwd {T}x{H}", median_ms(lambda: F.rms_norm(x, (H,), g, 1e-5), flush=True), 2 * T * H * 2)
+    _, mean, rstd_ln, _ = _C.layernorm_fwd(x, None, g, b, 1e-5, False)
+    _, _, rstd, _ = _C.layernorm_fwd(x, None, g, None, 1e-5, False, rms=True)
+    dg, db = torch.zeros(H, device=dev), torch.zeros(H, device=dev)
+    row(f"rmsnorm bwd {T}x{H}", median_ms(lambda: _C.layernorm_bwd(dy, x, g, None, rstd, None, dg, None, rms=True),
+                                          flush=True), 3 * T * H * 2)
+    row(f"layernorm bwd {T}x{H}", median_ms(lambda: _C.layernorm_bwd(dy, x, g, mean, rstd_ln, None, dg, db),
+                                            flush=True), 3 * T * H * 2)
+    xr, gr = x.clone().requires_grad_(), g.clone().requires_grad_()
+    yr = F.rms_norm(xr, (H,), gr, 1e-5)
+    row(f"F.rms_norm(lib) bwd {T}x{H}", median_ms(lambda: torch.autograd.grad(yr, (xr, gr), dy, retain_graph=True),
+                                                  flush=True), 3 * T * H * 2)
+
+    qkv = torch.randn(LLAMA_B, LLAMA_S, Hkv, G + 2, D, device=dev, dtype=bf)
+    pos = torch.arange(LLAMA_S, device=dev).repeat(LLAMA_B, 1)
+    nbytes = 2 * qkv.numel() * 2
+    row(f"rotary fwd B{LLAMA_B} S{LLAMA_S} Hq{Hq} Hkv{Hkv} D{D}",
+        median_ms(lambda: ops.rotary_packed(qkv, pos, 10000.0, False), flush=True), nbytes)
+    inv = P._inv_freq(D, 10000.0, str(qkv.device))
+    q = torch.randn(LLAMA_B, LLAMA_S, Hq, D, device=dev, dtype=bf).transpose(1, 2)   # HF's [B, heads, S, D] views
+    k = torch.randn(LLAMA_B, LLAMA_S, Hkv, D, device=dev, dtype=bf).transpose(1, 2)
+
+    def hf_rotary():
+        freqs = (inv[None, :, None].expand(LLAMA_B, -1, 1) @ pos[:, None, :].float()).transpose(1, 2)
+        emb = torch.cat((freqs, freqs), dim=-1)
+        return apply_rotary_pos_emb(q, k, emb.cos().to(bf), emb.sin().to(bf))
+    row("HF apply_rotary_pos_emb(lib) q+k incl. cos/sin", median_ms(hf_rotary, flush=True),
+        2 * (q.numel() + k.numel()) * 2)
+
+    gu = torch.randn(T, I, 2, device=dev, dtype=bf)
+    dh = torch.randn(T, I, device=dev, dtype=bf)
+    row(f"swiglu fwd {T}x{I}", median_ms(lambda: ops.swiglu(gu), flush=True), T * I * 6)
+    row(f"F.silu(g)*u(lib) fwd {T}x{I}", median_ms(lambda: F.silu(gu[..., 0]) * gu[..., 1], flush=True), T * I * 6)
+    row(f"swiglu bwd {T}x{I}", median_ms(lambda: ops.swiglu_bwd(dh, gu), flush=True), T * I * 10)
+    gur = gu.clone().requires_grad_()
+    hr = F.silu(gur[..., 0]) * gur[..., 1]
+    row(f"F.silu(g)*u(lib) bwd {T}x{I}", median_ms(lambda: torch.autograd.grad(hr, gur, dh, retain_graph=True),
+                                                   flush=True), T * I * 10)
+
+
+def sec_llama_step():
+    """One-GPU training of the 1.3B-sized Llama-style config through ShardParallel (fused AdamW on fp32 masters, as
+    bench.py trains GPT-1.3B): ms per step from CUDA events, the RMSNorm (with its dgamma reduction) / rotary / SwiGLU
+    kernels' share of one profiled step, and the library fallbacks (none expected)."""
+    import alpa_b200 as alpa
+    from alpa_b200.model.gpt_model import GPTConfig, GPTModel, gpt_lm_loss, num_params
+    from alpa_b200.model.model_util import TrainState, adamw, functional_call, params_of
+    alpa.init(cluster="local")
+    cfg = GPTConfig(arch="llama", vocab_size=51200, hidden_size=LLAMA_H, num_hidden_layers=24,
+                    num_attention_heads=LLAMA_HQ, num_key_value_heads=LLAMA_HKV, intermediate_size=LLAMA_I,
+                    causal=True, layer_norm_eps=1e-5, dtype=torch.bfloat16)
+    model = GPTModel(cfg, device=dev)
+    state = TrainState.create(apply_fn=None, params=params_of(model), use_master_copy=True, tx=adamw(1e-4, fused=True))
+
+    def train_step(state, batch):
+        def loss_fn(p):
+            return gpt_lm_loss(functional_call(model, p, (batch["input_ids"], batch["position_ids"])), batch["labels"])
+        loss, grads = alpa.value_and_grad(loss_fn)(state.params)
+        return state.apply_gradients(grads=grads), loss
+
+    step = alpa.parallelize(train_step, method=alpa.ShardParallel(), donate_argnums=(0,))
+    B, S = LLAMA_B, LLAMA_S
+    batch = {"input_ids": torch.randint(1, cfg.vocab_size, (B, S), device=dev),
+             "position_ids": torch.arange(S, device=dev).repeat(B, 1),
+             "labels": torch.randint(1, cfg.vocab_size, (B, S), device=dev)}
+    losses = []
+    for _ in range(3):
+        state, loss = step(state, batch)
+    torch.cuda.synchronize()
+    n = 10
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(n):
+        state, loss = step(state, batch)
+        losses.append(loss)
+    e1.record()
+    torch.cuda.synchronize()
+    ms = e0.elapsed_time(e1) / n
+    print(f"BENCH llama_step {num_params(cfg) / 1e9:.2f}B params, B{B} S{S}: {ms:.1f} ms/step, "
+          f"{B * S / ms * 1e3:.0f} tokens/s, losses {float(losses[0]._value):.4f} -> {float(losses[-1]._value):.4f}",
+          flush=True)
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        state, loss = step(state, batch)
+        torch.cuda.synchronize()
+    total, share = 0.0, {}
+    for ev in prof.key_averages():
+        t = ev.device_time_total if hasattr(ev, "device_time_total") else ev.cuda_time_total
+        total += t
+        name = ev.key
+        # reduce_slots_kernel sums the RMSNorm backward's dgamma slots; its other users (bias gradients, grad-norm
+        # clipping) do not run in this step, which is checked below
+        kind = ("rotary" if "rotary_packed_kernel" in name else "swiglu" if "swiglu_" in name else
+                "rmsnorm" if ("layernorm" in name and "true>" in name) or "reduce_slots_kernel" in name else None)
+        if kind:
+            share[kind] = share.get(kind, 0.0) + t
+        if "colsum_kernel" in name or "sumsq_kernel" in name:
+            FAILS.append(f"llama_step: {name} also uses reduce_slots_kernel; the RMSNorm share would include it")
+    for kind, t in sorted(share.items()):
+        print(f"BENCH llama_step kernel share {kind}: {t / 1e3:.2f} ms of {total / 1e3:.2f} ms GPU time "
+              f"({100 * t / total:.1f} %)", flush=True)
+    fb = P.library_fallbacks()
+    print(f"llama_step library_fallbacks: {fb}", flush=True)
+    if fb:
+        FAILS.append("llama_step library fallbacks")
+    alpa.shutdown()
+
+
 SECTIONS = {"gemm_bench": sec_gemm_bench, "gemm_sweep": sec_gemm_sweep, "misc": sec_misc, "attn": sec_attn,
-            "attn_gqa": sec_attn_gqa, "moe": sec_moe, "fp8": sec_fp8, "gemv": sec_gemv, "ragged": sec_ragged}
+            "attn_gqa": sec_attn_gqa, "moe": sec_moe, "fp8": sec_fp8, "gemv": sec_gemv, "ragged": sec_ragged,
+            "llama": sec_llama, "llama_step": sec_llama_step}
 
 
 def card():
