@@ -1,4 +1,4 @@
-"""Decoder-only LMs for serving: OPT, BLOOM and CodeGen variants of one tensor-parallel transformer.
+"""Decoder-only LMs for serving: OPT, BLOOM, CodeGen and Llama variants of one tensor-parallel transformer.
 
 Reference: examples/llm_serving/model/opt_model.py (OPTConfig:44, OPTEmbeddings:95, OPTSelfAttention:138 with the
 KV cache threaded through `attention_cache`, OPTTransformerLayer:316, OPTForLMModule:470, get_opt_config:533,
@@ -10,6 +10,11 @@ explicitly (column-parallel QKV / FC1, row-parallel out-proj / FC2, vocab-parall
 all-reduces on the NVSwitch (NCCL / NVLS), KV cache resident in HBM as [B, S_max, heads_local, D] per layer, the
 prompt phase on the flash-attention kernel and every decode step replayed from a CUDA graph.  Weights can be kept in
 fp8 (e4m3, per-output-channel scales) to halve the weight traffic that bounds decode.
+
+`arch="llama"` serves the Llama-style model of `gpt_model.GPTModel(arch="llama")` from its parameters: pre-RMSNorm
+blocks without biases, grouped-query attention with rotary embeddings, a SwiGLU MLP.  Its KV cache holds only the K/V
+heads ([B, S_max, Hkv_local, D]); a decode step rotates, appends and attends in one kernel that reads each K/V row once
+for its whole group of query heads.
 """
 from __future__ import annotations
 
@@ -27,7 +32,7 @@ from alpa_b200 import ops
 @dataclass
 class OPTConfig:
     """(reference: OPTConfig, opt_model.py:44-77; bloom/codegen configs share the fields)"""
-    arch: str = "opt"                     # opt | bloom | codegen
+    arch: str = "opt"                     # opt | bloom | codegen | llama
     vocab_size: int = 50272
     hidden_size: int = 768
     num_hidden_layers: int = 12
@@ -44,12 +49,24 @@ class OPTConfig:
     tie_word_embeddings: Optional[bool] = None
     dtype: torch.dtype = torch.bfloat16
     weight_dtype: str = "bf16"            # bf16 | fp8 (e4m3 weights, per-channel scales) | mxfp8 (e4m3 + UE8M0 per 32)
+    # llama: K/V heads of grouped-query attention (None = num_attention_heads) and the rotary base; layer_norm_eps is
+    # the RMSNorm eps and ffn_dim the SwiGLU width
+    num_key_value_heads: Optional[int] = None
+    rope_theta: float = 10000.0
 
     def __post_init__(self):
         if self.parallel_block is None:
             self.parallel_block = self.arch == "codegen"
         if self.tie_word_embeddings is None:
-            self.tie_word_embeddings = self.arch != "codegen"
+            self.tie_word_embeddings = self.arch not in ("codegen", "llama")
+        if self.num_attention_heads % self.kv_heads:
+            raise ValueError("num_key_value_heads must divide num_attention_heads")
+        if self.arch != "llama" and self.kv_heads != self.num_attention_heads:
+            raise ValueError(f"grouped-query attention is served for arch='llama' only, not {self.arch!r}")
+
+    @property
+    def kv_heads(self):
+        return self.num_key_value_heads or self.num_attention_heads
 
     @property
     def head_dim(self):
@@ -66,11 +83,21 @@ BLOOM_SPECS = {"560m": (24, 1024, 16), "1b7": (24, 2048, 16), "3b": (30, 2560, 3
                "176b": (70, 14336, 112)}
 CODEGEN_SPECS = {"350m": (20, 1024, 16), "2b": (32, 2560, 32), "6b": (33, 4096, 16), "16b": (34, 6144, 24)}
 CODEGEN_ROTARY = {"350m": 32, "2b": 64, "6b": 64, "16b": 64}          # (reference: codegen_model.py:514-537)
+# name -> (layers, hidden, heads, kv heads, ffn, vocab, rope theta, max positions) of the Hugging Face configs
+LLAMA_SPECS = {"2-7b": (32, 4096, 32, 32, 11008, 32000, 10000.0, 4096),
+               "2-70b": (80, 8192, 64, 8, 28672, 32000, 10000.0, 4096),
+               "3-8b": (32, 4096, 32, 8, 14336, 128256, 500000.0, 8192)}
 
 
 def get_config(name: str, **kw) -> OPTConfig:
-    """'opt-2.7b', 'bloom-7b1', 'codegen-2b' ... (reference: get_opt_config / get_bloom_config / get_codegen_config)"""
-    fam, _, size = name.lower().replace("facebook/", "").replace("alpa/", "").partition("-")
+    """'opt-2.7b', 'bloom-7b1', 'codegen-2b', 'llama-3-8b' ... (reference: get_opt_config / get_bloom_config /
+    get_codegen_config)"""
+    fam, _, size = name.lower().replace("facebook/", "").replace("alpa/", "").replace("meta-llama/", "").partition("-")
+    if fam == "llama":
+        L, H, nh, kv, I, V, theta, S = LLAMA_SPECS[size.replace("llama-", "").removesuffix("-hf")]
+        return OPTConfig(arch="llama", vocab_size=V, hidden_size=H, num_hidden_layers=L, num_attention_heads=nh,
+                         num_key_value_heads=kv, ffn_dim=I, max_position_embeddings=S, rope_theta=theta,
+                         pad_token_id=0, activation="silu", **kw)
     if fam == "opt":
         L, H, nh = OPT_SPECS[size]
         return OPTConfig(arch="opt", vocab_size=50272, hidden_size=H, num_hidden_layers=L, num_attention_heads=nh,
@@ -85,6 +112,31 @@ def get_config(name: str, **kw) -> OPTConfig:
         return OPTConfig(arch="codegen", vocab_size=51200, hidden_size=H, num_hidden_layers=L, num_attention_heads=nh,
                          ffn_dim=4 * H, activation="gelu", rotary_dim=CODEGEN_ROTARY[size], **kw)
     raise ValueError(name)
+
+
+def serving_config_from_gpt(gcfg, **kw) -> OPTConfig:
+    """The serving config of a `GPTConfig(arch="llama")` (e.g. from `llama_config_from_hf`); `kw` overrides fields
+    (dtype, weight_dtype, ...)."""
+    if gcfg.arch != "llama":
+        raise ValueError(f"only arch='llama' GPT configs are served, not {gcfg.arch!r}")
+    args = dict(arch="llama", vocab_size=gcfg.vocab_size, hidden_size=gcfg.hidden_size,
+                num_hidden_layers=gcfg.num_hidden_layers, num_attention_heads=gcfg.num_attention_heads,
+                num_key_value_heads=gcfg.num_key_value_heads or gcfg.num_attention_heads,
+                ffn_dim=gcfg.intermediate_size, max_position_embeddings=gcfg.max_position_embeddings,
+                layer_norm_eps=gcfg.layer_norm_eps, pad_token_id=0, activation="silu",
+                tie_word_embeddings=gcfg.tie_word_embeddings, rope_theta=gcfg.rope_theta, dtype=gcfg.dtype)
+    args.update(kw)
+    return OPTConfig(**args)
+
+
+def gpt_config_from_serving(cfg: OPTConfig):
+    """The `GPTConfig(arch="llama")` whose parameter layout `DecoderLM(cfg)` takes."""
+    from alpa_b200.model.gpt_model import GPTConfig
+    return GPTConfig(arch="llama", vocab_size=cfg.vocab_size, hidden_size=cfg.hidden_size,
+                     num_hidden_layers=cfg.num_hidden_layers, num_attention_heads=cfg.num_attention_heads,
+                     num_key_value_heads=cfg.num_key_value_heads, intermediate_size=cfg.ffn_dim,
+                     max_position_embeddings=cfg.max_position_embeddings, layer_norm_eps=cfg.layer_norm_eps,
+                     tie_word_embeddings=cfg.tie_word_embeddings, rope_theta=cfg.rope_theta, dtype=cfg.dtype)
 
 
 class _TPLinear:
@@ -109,18 +161,19 @@ class _TPLinear:
 
     def __call__(self, x: torch.Tensor, act: str = "none", residual: Optional[torch.Tensor] = None,
                  ln=None) -> torch.Tensor:
-        """`ln` = (gamma, beta, eps): layer-normalise x first (fused into the decode GEMV's prologue)."""
+        """`ln` = (gamma, beta, eps) or ops.RMSNormArgs(gamma, eps): normalise x first (fused into the decode GEMV's
+        prologue)."""
         rows = x.numel() // x.shape[-1]
         if self.mx:
             if ln is not None:
-                x = ops.fast.layer_norm(x, ln[0], ln[1], ln[2])[0]
+                x = ops.fast.norm_rows(x, ln)
             y = ops.fast.linear_mxfp8(x, self.w, self.scale, self.b, act)
             return y if residual is None else y + residual
         if rows <= 8 and x.is_cuda and x.dtype == torch.bfloat16:
             # decode: weight-streaming GEMV (no activation quantisation, no tile padding), LN / residual fused
             return ops.fast.linear_decode(x, self.w, self.scale, self.b, act, residual, ln)
         if ln is not None:
-            x = ops.fast.layer_norm(x, ln[0], ln[1], ln[2])[0]
+            x = ops.fast.norm_rows(x, ln)
         if residual is not None:
             return self(x, act) + residual
         if self.fp8:
@@ -159,8 +212,12 @@ class DecoderLM:
         self.tp = dist.get_world_size(group) if group is not None else 1
         self.rank = dist.get_rank(group) if group is not None else 0
         H, I, nh, V = cfg.hidden_size, cfg.ffn_dim, cfg.num_attention_heads, cfg.vocab_size
+        if cfg.arch == "llama" and cfg.kv_heads % self.tp:
+            raise ValueError(f"tensor parallelism over {self.tp} ranks needs num_key_value_heads "
+                             f"({cfg.kv_heads}) to be a multiple of it")
         assert nh % self.tp == 0 and I % self.tp == 0
         self.nh_local = nh // self.tp
+        self.kv_local = cfg.kv_heads // self.tp           # K/V heads of this rank (= nh_local but for GQA)
         self.D = cfg.head_dim
         self.Vp = (V + 8 * self.tp - 1) // (8 * self.tp) * (8 * self.tp)      # padded so every shard is a multiple of 8
         self.V_local = self.Vp // self.tp
@@ -183,6 +240,10 @@ class DecoderLM:
 
         dev = self.device
         r, tp = self.rank, self.tp
+        self.alibi = None
+        if cfg.arch == "llama":
+            self._init_llama(params, rnd, fp8)
+            return
         wte = get("embed_tokens", V, H)
         wte = F.pad(wte, (0, 0, 0, self.Vp - V))
         self.wte = wte[r * self.V_local:(r + 1) * self.V_local].contiguous().to(dev)     # vocab-parallel, tied head
@@ -222,10 +283,50 @@ class DecoderLM:
             self.head_b = hb[r * self.V_local:(r + 1) * self.V_local].contiguous().to(dev)
         self.alibi = _alibi_slopes(nh)[r * self.nh_local:(r + 1) * self.nh_local].to(dev) if cfg.arch == "bloom" else None
 
+    def _init_llama(self, params, rnd, fp8):
+        """Weights of `GPTModel(arch="llama")` (its state_dict names and layouts), sliced for this rank: the QKV rows
+        (K/V head, {G query heads, k, v}, D) and the interleaved (gate, up) rows of fc1 split by columns, the
+        out-projection and fc2 by rows, the embedding and head by vocabulary."""
+        cfg, dev, r, tp = self.cfg, self.device, self.rank, self.tp
+        H, I, V, D = cfg.hidden_size, cfg.ffn_dim, cfg.vocab_size, self.D
+        G = cfg.num_attention_heads // cfg.kv_heads
+        std = 0.02
+
+        def get(name, *shape, ones=False):
+            if params is not None:
+                return torch.as_tensor(params[name]).to(cfg.dtype)
+            return torch.ones(*shape, dtype=cfg.dtype) if ones else rnd(*shape, std=std)
+
+        def rows(t, n):                   # this rank's n rows of a column-parallel weight
+            return t[r * n:(r + 1) * n].contiguous().to(dev)
+
+        wte = F.pad(get("wte", V, H), (0, 0, 0, self.Vp - V))
+        self.wte = rows(wte, self.V_local)
+        self.wpe, self.emb_ln, self.pos_offset = None, None, 0
+        eps = cfg.layer_norm_eps
+        self.layers = []
+        qkv_local, hl, il = self.kv_local * (G + 2) * D, self.nh_local * D, I // tp
+        for i in range(cfg.num_hidden_layers):
+            p = f"blocks.{i}."
+            self.layers.append({
+                "ln1": ops.RMSNormArgs(get(p + "ln1_g", H, ones=True).to(dev), eps),
+                "ln2": ops.RMSNormArgs(get(p + "ln2_g", H, ones=True).to(dev), eps),
+                "qkv": _TPLinear(rows(get(p + "qkv_w", (G + 2) * cfg.kv_heads * D, H), qkv_local), None, fp8),
+                "out": _TPLinear(get(p + "proj_w", H, H)[:, r * hl:(r + 1) * hl].contiguous().to(dev), None, fp8),
+                "fc1": _TPLinear(rows(get(p + "fc1_w", 2 * I, H), 2 * il), None, fp8),
+                "fc2": _TPLinear(get(p + "fc2_w", H, I)[:, r * il:(r + 1) * il].contiguous().to(dev), None, fp8),
+            })
+        self.final_ln = ops.RMSNormArgs(get("ln_f_g", H, ones=True).to(dev), eps)
+        if cfg.tie_word_embeddings:
+            self.head_w = self.wte
+        else:
+            self.head_w = rows(F.pad(get("decoder_w", V, H), (0, 0, 0, self.Vp - V)), self.V_local)
+        self.head_b = None
+
     # ------------------------------------------------------------------ cache
     def init_cache(self, batch_size: int, max_len: int):
-        """(reference: init_cache_np, opt_model.py:756) -> list of (k, v) [B, max_len, heads_local, D]"""
-        shape = (batch_size, max_len, self.nh_local, self.D)
+        """(reference: init_cache_np, opt_model.py:756) -> list of (k, v) [B, max_len, kv_heads_local, D]"""
+        shape = (batch_size, max_len, self.kv_local, self.D)
         return [(torch.zeros(shape, dtype=self.cfg.dtype, device=self.device),
                  torch.zeros(shape, dtype=self.cfg.dtype, device=self.device)) for _ in self.layers]
 
@@ -324,6 +425,8 @@ class DecoderLM:
         x = self._embed(input_ids, position_ids)
         scale = 1.0 / math.sqrt(self.D)
         end = cache_len + T
+        if cfg.arch == "llama":
+            return self._forward_llama(x, position_ids, cache, cache_len, last_only)
         for l, (kc, vc) in zip(self.layers, cache):
             h = ops.fast.layer_norm(x, l["ln1"][0], l["ln1"][1], cfg.layer_norm_eps)[0]
             qkv = l["qkv"](h).view(B, T, self.nh_local, 3, self.D)
@@ -349,6 +452,36 @@ class DecoderLM:
         x = ops.fast.layer_norm(x.contiguous(), self.final_ln[0], self.final_ln[1], cfg.layer_norm_eps)[0]
         return ops.fast.linear(x, self.head_w, self.head_b)
 
+    def _mlp_llama(self, l, h):
+        gu = l["fc1"](h)
+        return l["fc2"](ops.fast.swiglu(gu.view(*gu.shape[:-1], gu.shape[-1] // 2, 2)))
+
+    def _forward_llama(self, x, position_ids, cache, cache_len, last_only):
+        cfg = self.cfg
+        B, T = x.shape[:2]
+        G = cfg.num_attention_heads // cfg.kv_heads
+        scale = 1.0 / math.sqrt(self.D)
+        end = cache_len + T
+        for l, (kc, vc) in zip(self.layers, cache):
+            h = ops.fast.norm_rows(x, l["ln1"])
+            qkv = l["qkv"](h).view(B, T, self.kv_local, G + 2, self.D)
+            qkv = ops.fast.rotary_packed(qkv, position_ids, cfg.rope_theta, False)
+            kc[:, cache_len:end] = qkv[:, :, :, G]
+            vc[:, cache_len:end] = qkv[:, :, :, G + 1]
+            # the grouped Q view against the valid cache rows: causal with Sq != Sk
+            o, _ = ops.fast.attention(qkv[:, :, :, :G], kc[:, :end], vc[:, :end], scale, True)
+            x = x + self._all_reduce(l["out"](o.reshape(B, T, self.nh_local * self.D)))
+            x = x + self._all_reduce(self._mlp_llama(l, ops.fast.norm_rows(x, l["ln2"])))
+        if last_only:
+            x = x[:, -1:]
+        return self._head_llama(ops.fast.norm_rows(x.contiguous(), self.final_ln))
+
+    def _head_llama(self, x):
+        """The LM head: the weight-streaming GEMV for the few rows of a prefill's last tokens, else the GEMM."""
+        if x.numel() // x.shape[-1] <= 8:
+            return ops.fast.linear_decode(x, self.head_w, None)
+        return ops.fast.linear(x, self.head_w, None)
+
     def decode_step(self, input_ids: torch.Tensor, position_ids: torch.Tensor, cache, kv_len: torch.Tensor) -> torch.Tensor:
         """One new token per sequence with every position-dependent quantity on the device: `position_ids` [B, 1]
         (int64) is both the embedding position and the cache row to write, `kv_len` (int32 scalar tensor) the number
@@ -360,6 +493,23 @@ class DecoderLM:
         x = self._embed(input_ids, position_ids)
         scale = 1.0 / math.sqrt(self.D)
         eps = cfg.layer_norm_eps
+        if cfg.arch == "llama":
+            G = cfg.num_attention_heads // cfg.kv_heads
+            for l, (kc, vc) in zip(self.layers, cache):
+                # 5 launches per layer (7 under tensor parallelism): RMSNorm in the QKV / fc1 GEMV prologues, rotary and
+                # the cache append in the attention kernel, residual adds in the GEMV / all-reduce epilogues
+                qkv = l["qkv"](x, ln=l["ln1"]).view(B, 1, self.kv_local, G + 2, self.D)
+                o = ops.fast.decode_attention_gqa(qkv, kc, vc, kv_len, position_ids, scale, cfg.rope_theta)
+                o = o.reshape(B, 1, self.nh_local * self.D)
+                if self.tp == 1:
+                    x = l["out"](o, residual=x)
+                    gu = l["fc1"](x, ln=l["ln2"])
+                    x = l["fc2"](ops.fast.swiglu(gu.view(B, 1, -1, 2)), residual=x)
+                else:
+                    x = self._all_reduce(l["out"](o), residual=x)
+                    gu = l["fc1"](x, ln=l["ln2"])
+                    x = self._all_reduce(l["fc2"](ops.fast.swiglu(gu.view(B, 1, -1, 2))), residual=x)
+            return ops.fast.linear_decode(x.contiguous(), self.head_w, None, None, ln=self.final_ln)
         for l, (kc, vc) in zip(self.layers, cache):
             # 5 launches per layer (7 under tensor parallelism): LN rides in the GEMV prologues, the cache append in
             # the attention kernel, residual adds in the GEMV / all-reduce epilogues
@@ -390,7 +540,7 @@ class DecoderLM:
     def init_cache_1d(self, num_slots: int):
         """Slot-addressed cache: per layer (k, v) of [num_slots + 1, heads_local, D]; the last row is the scratch row
         padding tokens write to.  (reference: init_cache_np of opt_model_1d.py:457 -- a 1-D token cache)"""
-        shape = (num_slots + 1, self.nh_local, self.D)
+        shape = (num_slots + 1, self.kv_local, self.D)
         return [(torch.zeros(shape, dtype=self.cfg.dtype, device=self.device),
                  torch.zeros(shape, dtype=self.cfg.dtype, device=self.device)) for _ in self.layers]
 
@@ -406,6 +556,18 @@ class DecoderLM:
         x = self._embed(input_ids.view(1, T), position.view(1, T))[0]          # [T, H]
         scale = 1.0 / math.sqrt(self.D)
         alibi = self.alibi.float().contiguous() if self.alibi is not None else None
+        if cfg.arch == "llama":
+            G = cfg.num_attention_heads // cfg.kv_heads
+            for l, (kc, vc) in zip(self.layers, cache):
+                qkv = l["qkv"](ops.fast.norm_rows(x, l["ln1"])).view(1, T, self.kv_local, G + 2, self.D)
+                qkv = ops.fast.rotary_packed(qkv, position.view(1, T), cfg.rope_theta, False)[0]
+                kc.index_copy_(0, slot, qkv[:, :, G].contiguous())
+                vc.index_copy_(0, slot, qkv[:, :, G + 1].contiguous())
+                q = qkv[:, :, :G].reshape(T, self.nh_local, self.D)
+                o = ops.fast.ragged_attention(q, kc, vc, seq_start, ctx_len, scale, max_ctx)
+                x = x + self._all_reduce(l["out"](o.reshape(T, self.nh_local * self.D)))
+                x = x + self._all_reduce(self._mlp_llama(l, ops.fast.norm_rows(x, l["ln2"])))
+            return self._head_llama(ops.fast.norm_rows(x.index_select(0, logit_index).contiguous(), self.final_ln))
         for l, (kc, vc) in zip(self.layers, cache):
             h = ops.fast.layer_norm(x, l["ln1"][0], l["ln1"][1], cfg.layer_norm_eps)[0]
             qkv = l["qkv"](h).view(T, self.nh_local, 3, self.D)

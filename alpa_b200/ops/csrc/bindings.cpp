@@ -334,7 +334,8 @@ Tensor ragged_attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_
               v_cache.scalar_type() == at::kBFloat16, "ragged_attention: caches must be bf16 [slots, heads, D]");
   TORCH_CHECK(k_cache.stride(2) == 1 && k_cache.stride(1) == k_cache.size(2) && v_cache.strides() == k_cache.strides() &&
               v_cache.sizes() == k_cache.sizes(), "ragged_attention: cache rows must be dense");
-  TORCH_CHECK(k_cache.size(1) == q.size(1) && k_cache.size(2) == q.size(2));
+  TORCH_CHECK(k_cache.size(1) > 0 && q.size(1) % k_cache.size(1) == 0 && k_cache.size(2) == q.size(2),
+              "ragged_attention: the cache's heads must divide q's heads (grouped-query attention), head dims equal");
   TORCH_CHECK(aligned(k_cache.data_ptr(), 16) && aligned(v_cache.data_ptr(), 16),
               "ragged_attention: cache bases must be 16-byte aligned (16-byte K loads)");
   TORCH_CHECK(seq_start.scalar_type() == at::kInt && ctx_len.scalar_type() == at::kInt && seq_start.is_contiguous() &&
@@ -357,6 +358,7 @@ Tensor ragged_attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_
   a.q_stride_t = q.stride(0); a.q_stride_h = q.stride(1); a.o_stride_t = o.stride(0);
   a.kv_stride_s = k_cache.stride(0);
   a.scale = (float)scale;
+  a.group = (int)(q.size(1) / k_cache.size(1));
   AB_CHECK_RC(ab_ragged_attention(&a, cur_stream()), "ab_ragged_attention");
   g_launches += 1;
   return o;
@@ -972,7 +974,7 @@ Tensor gemm_mxfp8(const Tensor& x, const Tensor& wq, const Tensor& w_sf, const O
 // Decode-step GEMV: x [M<=8, K] bf16, w [N, K] e4m3 (with w_scale [N]) or bf16.
 Tensor gemv_decode(const Tensor& x, const Tensor& w, const OptTensor& w_scale, const OptTensor& bias,
                    const OptTensor& residual, int64_t act, const OptTensor& ln_gamma, const OptTensor& ln_beta,
-                   double ln_eps) {
+                   double ln_eps, bool ln_rms) {
   TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.scalar_type() == at::kBFloat16 && x.stride(1) == 1 &&
                   reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0, "gemv_decode: x (16-byte aligned rows)");
   const bool fp8 = w.scalar_type() == at::kFloat8_e4m3fn;
@@ -998,7 +1000,14 @@ Tensor gemv_decode(const Tensor& x, const Tensor& w, const OptTensor& w_scale, c
     a.residual = bf16_ptr(residual);
     a.ldr = residual->stride(0);
   }
-  if (ln_gamma.has_value() && ln_gamma->defined()) {
+  if (ln_rms) {
+    TORCH_CHECK(ln_gamma.has_value() && ln_gamma->defined() && !(ln_beta.has_value() && ln_beta->defined()) &&
+                ln_gamma->scalar_type() == at::kBFloat16 && ln_gamma->is_contiguous() && ln_gamma->numel() == a.K &&
+                aligned(ln_gamma->data_ptr(), 16), "gemv_decode: RMSNorm gamma must be bf16 [K] and beta absent");
+    a.ln_gamma = bf16_ptr(ln_gamma);
+    a.ln_eps = (float)ln_eps;
+    a.ln_rms = 1;
+  } else if (ln_gamma.has_value() && ln_gamma->defined()) {
     TORCH_CHECK(ln_beta.has_value() && ln_beta->defined() && ln_gamma->scalar_type() == at::kBFloat16 &&
                 ln_beta->scalar_type() == at::kBFloat16 && ln_gamma->is_contiguous() && ln_beta->is_contiguous() &&
                 ln_gamma->numel() == a.K && ln_beta->numel() == a.K, "gemv_decode: layer-norm gamma / beta must be bf16 [K]");
@@ -1009,6 +1018,28 @@ Tensor gemv_decode(const Tensor& x, const Tensor& w, const OptTensor& w_scale, c
   AB_CHECK_RC(ab_gemv_decode(&a, cur_stream()), "ab_gemv_decode");
   g_launches += 1;
   return y;
+}
+
+// Splits the key range of every CTA row so that ~2 CTAs per SM stream the cache (the length is only known on the
+// device), at most `max_splits`, and launches ab_decode_attention with its workspace and arrival counters.
+void launch_decode_attention(ab::DecodeAttnArgs& a, int max_splits, const Tensor& like) {
+  const int rows = a.B * ab_decode_attention_rows(&a);
+  a.splits = std::max(1, std::min(max_splits, (2 * ab::num_sms() + rows - 1) / rows));
+  Tensor ws;
+  if (a.splits > 1) {
+    // arrival counters: one persistent zeroed buffer per device; the merging CTA resets its counter
+    static std::unordered_map<int, Tensor> counters;
+    const int dev = like.get_device();
+    auto it = counters.find(dev);
+    if (it == counters.end() || it->second.numel() < rows)
+      it = counters.insert_or_assign(dev, torch::zeros({std::max(rows, 4096)}, like.options().dtype(at::kInt))).first;
+    a.counters = it->second.data_ptr<int>();
+    ws = torch::empty({(int64_t)rows * a.splits * ab_decode_attention_chunk(&a) * (a.D + 2)},
+                      like.options().dtype(at::kFloat));
+    a.ws = ws.data_ptr<float>();
+  }
+  AB_CHECK_RC(ab_decode_attention(&a, cur_stream()), "ab_decode_attention");
+  g_launches += 1;
 }
 
 // Decode-step attention, cache append fused: q / k_new / v_new [B, 1, heads, D] views, caches [B, S_max, heads, D].
@@ -1040,25 +1071,60 @@ Tensor decode_attention(const Tensor& q, const Tensor& k_new, const Tensor& v_ne
   a.new_stride_b = k_new.stride(0); a.new_stride_h = k_new.stride(2);
   a.cache_stride_b = k_cache.stride(0); a.cache_stride_s = k_cache.stride(1);
   a.scale = (float)scale;
+  a.kv_heads = a.heads;
   Tensor o = torch::empty({a.B, 1, a.heads, a.D}, q.options());
   a.o = reinterpret_cast<__nv_bfloat16*>(o.data_ptr());
-  // split the key range so that ~2 CTAs per SM stream the cache (the length is only known on the device)
-  const int bh = a.B * a.heads;
-  a.splits = std::max(1, std::min(16, (2 * ab::num_sms() + bh - 1) / bh));
-  Tensor ws;
-  if (a.splits > 1) {
-    // arrival counters: one persistent zeroed buffer per device; the merging CTA resets its counter
-    static std::unordered_map<int, Tensor> counters;
-    const int dev = q.get_device();
-    auto it = counters.find(dev);
-    if (it == counters.end() || it->second.numel() < bh)
-      it = counters.insert_or_assign(dev, torch::zeros({std::max(bh, 4096)}, q.options().dtype(at::kInt))).first;
-    a.counters = it->second.data_ptr<int>();
-    ws = torch::empty({(int64_t)bh * a.splits * (a.D + 2)}, q.options().dtype(at::kFloat));
-    a.ws = ws.data_ptr<float>();
+  launch_decode_attention(a, 16, q);
+  return o;
+}
+
+// Grouped-query decode over the packed QKV row of the new token, qkv_new [B, 1, Hkv, G + 2, D] (G query heads, k, v per
+// K/V head), caches [B, S_max, Hkv, D]; with position_ids [B, 1] int64 and inv_freq [D / 2] fp32 the query heads and
+// the new key are rotated first (HF's rotate_half) and the rotated key is appended.  Returns o [B, 1, Hkv * G, D].
+Tensor decode_attention_packed(const Tensor& qkv, Tensor k_cache, Tensor v_cache, const Tensor& kv_len, double scale,
+                               const OptTensor& position_ids, const OptTensor& inv_freq) {
+  TORCH_CHECK(qkv.is_cuda() && qkv.dim() == 5 && qkv.size(1) == 1 && qkv.size(3) >= 3 &&
+                  qkv.scalar_type() == at::kBFloat16 && qkv.is_contiguous(),
+              "decode_attention_packed: qkv_new must be contiguous bf16 [B, 1, Hkv, G + 2, D]");
+  const int64_t B = qkv.size(0), Hkv = qkv.size(2), G = qkv.size(3) - 2, D = qkv.size(4);
+  TORCH_CHECK(k_cache.dim() == 4 && k_cache.scalar_type() == at::kBFloat16 && v_cache.scalar_type() == at::kBFloat16 &&
+              k_cache.sizes() == v_cache.sizes() && k_cache.strides() == v_cache.strides() && k_cache.size(0) == B &&
+              k_cache.size(2) == Hkv && k_cache.size(3) == D && k_cache.stride(3) == 1 && k_cache.stride(2) == D &&
+              k_cache.is_cuda() && k_cache.get_device() == qkv.get_device(),
+              "decode_attention_packed: caches must be bf16 [B, S_max, Hkv, D] on qkv's device, rows dense");
+  TORCH_CHECK(kv_len.is_cuda() && kv_len.scalar_type() == at::kInt && kv_len.numel() == 1,
+              "decode_attention_packed: kv_len must be an int32 CUDA scalar");
+  TORCH_CHECK(aligned(qkv.data_ptr(), 16) && aligned(k_cache.data_ptr(), 16) && aligned(v_cache.data_ptr(), 16),
+              "decode_attention_packed: qkv_new and the caches must start on 16-byte boundaries (16-byte accesses)");
+  const bool rope = position_ids.has_value() && position_ids->defined();
+  TORCH_CHECK(rope == (inv_freq.has_value() && inv_freq->defined()),
+              "decode_attention_packed: position_ids and inv_freq go together");
+  c10::cuda::CUDAGuard guard(qkv.device());
+  ab::DecodeAttnArgs a;
+  if (rope) {
+    TORCH_CHECK(position_ids->is_cuda() && position_ids->scalar_type() == at::kLong && position_ids->is_contiguous() &&
+                    position_ids->numel() == B && position_ids->get_device() == qkv.get_device(),
+                "decode_attention_packed: position_ids must be int64 [B, 1] on qkv's device");
+    TORCH_CHECK(inv_freq->is_cuda() && inv_freq->scalar_type() == at::kFloat && inv_freq->is_contiguous() &&
+                    inv_freq->numel() == D / 2 && D % 16 == 0 && inv_freq->get_device() == qkv.get_device(),
+                "decode_attention_packed: inv_freq must be fp32 [D / 2] on qkv's device, D a multiple of 16");
+    a.pos = position_ids->data_ptr<int64_t>();
+    a.inv_freq = inv_freq->data_ptr<float>();
   }
-  AB_CHECK_RC(ab_decode_attention(&a, cur_stream()), "ab_decode_attention");
-  g_launches += 1;
+  const __nv_bfloat16* base = bf16_ptr(qkv);
+  a.q = base; a.k_new = base + G * D; a.v_new = base + (G + 1) * D;
+  a.k_cache = reinterpret_cast<__nv_bfloat16*>(k_cache.data_ptr());
+  a.v_cache = reinterpret_cast<__nv_bfloat16*>(v_cache.data_ptr());
+  a.kv_len = kv_len.data_ptr<int>();
+  a.B = (int)B; a.kv_heads = (int)Hkv; a.group = (int)G; a.heads = (int)(Hkv * G); a.D = (int)D;
+  a.S_max = (int)k_cache.size(1);
+  a.q_stride_b = qkv.stride(0); a.q_stride_h = qkv.stride(2); a.q_stride_g = qkv.stride(3);
+  a.new_stride_b = qkv.stride(0); a.new_stride_h = qkv.stride(2);
+  a.cache_stride_b = k_cache.stride(0); a.cache_stride_s = k_cache.stride(1);
+  a.scale = (float)scale;
+  Tensor o = torch::empty({B, 1, Hkv * G, D}, qkv.options());
+  a.o = reinterpret_cast<__nv_bfloat16*>(o.data_ptr());
+  launch_decode_attention(a, 64, qkv);
   return o;
 }
 
@@ -1123,8 +1189,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("gemm_mxfp8_q", &gemm_mxfp8_q);
   m.def("gemv_decode", &gemv_decode, py::arg("x"), py::arg("w"), py::arg("w_scale") = py::none(),
         py::arg("bias") = py::none(), py::arg("residual") = py::none(), py::arg("act") = 0,
-        py::arg("ln_gamma") = py::none(), py::arg("ln_beta") = py::none(), py::arg("ln_eps") = 1e-5);
+        py::arg("ln_gamma") = py::none(), py::arg("ln_beta") = py::none(), py::arg("ln_eps") = 1e-5,
+        py::arg("ln_rms") = false);
   m.def("decode_attention", &decode_attention);
+  m.def("decode_attention_packed", &decode_attention_packed, py::arg("qkv_new"), py::arg("k_cache"), py::arg("v_cache"),
+        py::arg("kv_len"), py::arg("scale"), py::arg("position_ids") = py::none(), py::arg("inv_freq") = py::none());
   m.def("moe_top2_route", &moe_top2_route);
   m.def("moe_dispatch_", &moe_dispatch_, py::arg("x"), py::arg("expert"), py::arg("slot"), py::arg("weight"),
         py::arg("d"), py::arg("capacity"), py::arg("peer_ptrs") = std::vector<int64_t>(), py::arg("g_off") = 0);

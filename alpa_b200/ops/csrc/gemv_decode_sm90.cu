@@ -14,8 +14,9 @@
 //     2 global loads, 1 shared load and 2 MMAs.
 //   * n = 8 columns of the MMA are the (up to 8) tokens of the step.
 //   * fp8 weights: the activations are quantised per token to e4m3 in the prologue (same numerics as the prefill GEMM,
-//     gemm_sm90.cu); bf16 weights: bf16 activations.  The optional layer norm of x is fused into the same
-//     prologue: every CTA normalises / quantises the <= 8 rows itself (a few KB from L2) into shared memory.
+//     gemm_sm90.cu); bf16 weights: bf16 activations.  The optional layer norm (or RMSNorm, RMS = true) of x is fused
+//     into the same prologue: every CTA normalises / quantises the <= 8 rows itself (a few KB from L2) into shared
+//     memory.
 //   * split-K partials are reduced through shared memory; scale / bias / GELU | ReLU / residual in the epilogue.
 //   * the first weight loads are issued before the programmatic-dependent-launch wait (pdl.h).
 // Reference behaviour: the decode path of examples/llm_serving/model/opt_model.py (XLA cuBLAS GEMMs on fp16 weights).
@@ -68,7 +69,7 @@ __device__ __forceinline__ float block_max(float v, float* red, int warp, int la
   return t;
 }
 
-template <bool FP8>
+template <bool FP8, bool RMS>
 __global__ void __launch_bounds__(kGemvThreads) gemv_decode_kernel(const GemvArgs a) {
   constexpr int kEs = FP8 ? 1 : 2;            // bytes per weight / staged activation
   constexpr int kBlk = 64 / kEs;              // k per block: 16 bytes per lane quarter
@@ -109,7 +110,20 @@ __global__ void __launch_bounds__(kGemvThreads) gemv_decode_kernel(const GemvArg
   for (int m = 0; m < M; ++m) {
     const __nv_bfloat16* xrow = a.x + (size_t)m * a.ldx;
     float mean = 0.f, rstd = 1.f;
-    if (ln) {
+    if (RMS) {
+      // one pass: RMSNorm has no mean to subtract
+      float s2 = 0.f;
+      for (int i = threadIdx.x; i < xchunks; i += kGemvThreads) {
+        const int4 v = *reinterpret_cast<const int4*>(xrow + (size_t)i * 8);
+        const uint32_t* u = reinterpret_cast<const uint32_t*>(&v);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const float2 f = unpack_bf16x2(u[q]);
+          s2 = fmaf(f.x, f.x, fmaf(f.y, f.y, s2));
+        }
+      }
+      rstd = rsqrtf(block_sum(s2, red, warp, lane) / (float)K + a.ln_eps);
+    } else if (ln) {
       // two passes over the row (it stays in L1 / L2), like the stand-alone layer norm: s2/K - mean^2 cancels
       // catastrophically in fp32 when |mean| >> std
       float s1 = 0.f, s2 = 0.f;
@@ -138,7 +152,18 @@ __global__ void __launch_bounds__(kGemvThreads) gemv_decode_kernel(const GemvArg
     auto value8 = [&](int i, float* f) {      // 8 (normalised, bf16-rounded) activations of chunk i
       const int4 v = *reinterpret_cast<const int4*>(xrow + (size_t)i * 8);
       const uint32_t* u = reinterpret_cast<const uint32_t*>(&v);
-      if (ln) {
+      if (RMS) {
+        const int4 gv = *reinterpret_cast<const int4*>(a.ln_gamma + (size_t)i * 8);
+        const uint32_t* gu = reinterpret_cast<const uint32_t*>(&gv);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const float2 x2 = unpack_bf16x2(u[q]), g2 = unpack_bf16x2(gu[q]);
+          // round to bf16 like the stand-alone RMSNorm kernel does
+          const float2 r = unpack_bf16x2(pack_bf16x2(x2.x * rstd * g2.x, x2.y * rstd * g2.y));
+          f[2 * q] = r.x;
+          f[2 * q + 1] = r.y;
+        }
+      } else if (ln) {
         const int4 gv = *reinterpret_cast<const int4*>(a.ln_gamma + (size_t)i * 8);
         const int4 bv = *reinterpret_cast<const int4*>(a.ln_beta + (size_t)i * 8);
         const uint32_t* gu = reinterpret_cast<const uint32_t*>(&gv);
@@ -247,11 +272,11 @@ __global__ void __launch_bounds__(kGemvThreads) gemv_decode_kernel(const GemvArg
   }
 }
 
-template <bool FP8>
+template <bool FP8, bool RMS>
 static int gemv_launch(const GemvArgs& a, cudaStream_t st) {
   const int grid = (a.N + kGemvRows - 1) / kGemvRows;
   const size_t smem = (size_t)a.M * a.K * (FP8 ? 1 : 2);
-  auto kern = gemv_decode_kernel<FP8>;
+  auto kern = gemv_decode_kernel<FP8, RMS>;
   if (smem > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return 100 + (int)e;
@@ -267,6 +292,10 @@ extern "C" int ab_gemv_decode(const ab::GemvArgs* a, cudaStream_t st) {
   if (a->M < 1 || a->M > 8 || a->N <= 0) return 1;
   if (a->K % (a->fp8 ? 64 : 32) != 0 || a->ldx % 8 != 0) return 1;
   if ((size_t)a->M * a->K * (a->fp8 ? 1 : 2) > 200 * 1024) return 3;      // staged activations must fit shared memory
+  if (a->ln_rms) {
+    if (a->ln_gamma == nullptr || a->ln_beta != nullptr) return 3;
+    return a->fp8 ? gemv_launch<true, true>(*a, st) : gemv_launch<false, true>(*a, st);
+  }
   if (a->ln_gamma != nullptr && a->ln_beta == nullptr) return 3;
-  return a->fp8 ? gemv_launch<true>(*a, st) : gemv_launch<false>(*a, st);
+  return a->fp8 ? gemv_launch<true, false>(*a, st) : gemv_launch<false, false>(*a, st);
 }

@@ -88,6 +88,7 @@ struct GemvArgs {
   const __nv_bfloat16* ln_gamma = nullptr;
   const __nv_bfloat16* ln_beta = nullptr;
   float ln_eps = 1e-5f;
+  int ln_rms = 0;  // RMSNorm prologue instead (ln_beta null): y = x * rsqrt(mean(x^2) + eps) * gamma
 };
 
 struct AttnBwdArgs {
@@ -119,22 +120,31 @@ struct RaggedAttnArgs {
   int T = 0, heads = 0, D = 0, max_ctx = 0;
   long long q_stride_t = 0, q_stride_h = 0, o_stride_t = 0, kv_stride_s = 0;
   float scale = 1.f;
+  int group = 1;  // grouped-query attention: query head h reads cache head h / group of a [slots, heads / group, D] cache
 };
 
-// Decode-step attention with fused KV-cache append (decode_attention_sm90.cu)
+// Decode-step attention with fused KV-cache append (decode_attention_sm90.cu).  Grouped-query attention: query head
+// kv * group + g (g < group) attends with K/V head kv (HF's repeat_kv order); group == 1 is multi-head attention.
+// A CTA serves a chunk of up to 8 query heads of one K/V head (ab_decode_attention_rows: the CTA rows per sequence).
 struct DecodeAttnArgs {
-  const __nv_bfloat16* q = nullptr;        // [B, heads, D] view, D contiguous
-  const __nv_bfloat16* k_new = nullptr;    // [B, heads, D] views with one stride pair
+  const __nv_bfloat16* q = nullptr;        // [B, kv_heads, group, D] view, D contiguous
+  const __nv_bfloat16* k_new = nullptr;    // [B, kv_heads, D] views with one stride pair
   const __nv_bfloat16* v_new = nullptr;
-  __nv_bfloat16* k_cache = nullptr;        // [B, S_max, heads, D], heads*D dense inside a row
+  __nv_bfloat16* k_cache = nullptr;        // [B, S_max, kv_heads, D], kv_heads*D dense inside a row
   __nv_bfloat16* v_cache = nullptr;
-  __nv_bfloat16* o = nullptr;              // [B, heads, D] contiguous
+  __nv_bfloat16* o = nullptr;              // [B, heads, D] contiguous, heads = kv_heads * group
   const int* kv_len = nullptr;             // device scalar: valid rows including the new one
-  float* ws = nullptr;                     // [B, heads, splits, D + 2] fp32 partials (splits > 1)
-  int* counters = nullptr;                 // [B * heads] arrival counters, zero between launches
+  float* ws = nullptr;                     // [B, rows, splits, chunk, D + 2] fp32 partials (splits > 1)
+  int* counters = nullptr;                 // [B * rows] arrival counters, zero between launches
   int B = 0, heads = 0, D = 0, S_max = 0, splits = 1;
   long long q_stride_b = 0, q_stride_h = 0, new_stride_b = 0, new_stride_h = 0, cache_stride_b = 0, cache_stride_s = 0;
   float scale = 1.f;
+  int kv_heads = 0, group = 1;
+  long long q_stride_g = 0;                // between the query heads of one K/V head
+  // optional fused rotary embedding (HF's rotate_half) of the query heads and k_new before they are used:
+  // pos [B] int64 positions, inv_freq [D / 2] fp32; both null = none
+  const int64_t* pos = nullptr;
+  const float* inv_freq = nullptr;
 };
 
 // Sharding-invariant counter-based dropout (dropout_sm90.cu)
@@ -186,6 +196,8 @@ int ab_attention_bwd_splits(const ab::AttnArgs* a);  // parts the dK / dV kernel
 int ab_gemv_decode(const ab::GemvArgs* a, cudaStream_t st);
 int ab_ragged_attention(const ab::RaggedAttnArgs* a, cudaStream_t st);
 int ab_decode_attention(const ab::DecodeAttnArgs* a, cudaStream_t st);
+int ab_decode_attention_rows(const ab::DecodeAttnArgs* a);  // CTA rows per sequence (kv_heads * group chunks)
+int ab_decode_attention_chunk(const ab::DecodeAttnArgs* a);  // query heads per CTA (partials per row and split)
 int ab_dropout(const ab::DropoutArgs* a, int is_bf16, cudaStream_t st);
 int ab_rs_reduce(const __nv_bfloat16* staging, const uint32_t* flags, uint32_t expected, __nv_bfloat16* out,
                  const __nv_bfloat16* bias, const __nv_bfloat16* residual, int rows, int N, int tp,

@@ -3,7 +3,8 @@
 // Reference behaviour: examples/llm_serving/model/opt_model_1d.py:151-178 calls the external FasterTransformer
 // `fused_mmha(qkv, bias, cache_k, cache_v)` on a flat token batch whose tokens belong to different sequences.
 //
-// Layout here: q/o are [T, heads, D]; the KV cache is [slots, heads, D] and every sequence owns a contiguous slot
+// Layout here: q/o are [T, heads, D]; the KV cache is [slots, heads / group, D] (grouped-query attention: query head h
+// reads cache head h / group; group = 1 is multi-head attention) and every sequence owns a contiguous slot
 // range (alpa_b200/csrc/serving_runtime.cpp).  Token t attends to cache rows [seq_start[t], seq_start[t]+ctx_len[t])
 // -- prompt tokens and decode tokens look the same, causality is encoded in ctx_len.  One CTA per (head, token):
 //   pass 1  thread-per-key dot products with 16-byte K loads -> scores in shared memory, block max / sum
@@ -53,7 +54,8 @@ __global__ void __launch_bounds__(kRaggedThreads) ragged_attention_kernel(Ragged
   __syncthreads();
 
   const float slope = a.alibi ? a.alibi[head] : 0.f;
-  const __nv_bfloat16* kbase = a.k_cache + row0 * a.kv_stride_s + (long long)head * D;
+  const int kv_head = head / a.group;
+  const __nv_bfloat16* kbase = a.k_cache + row0 * a.kv_stride_s + (long long)kv_head * D;
   float lmax = -INFINITY;
   for (int j = tid; j < ctx; j += kRaggedThreads) {
     const int4* kr = reinterpret_cast<const int4*>(kbase + (long long)j * a.kv_stride_s);
@@ -89,7 +91,7 @@ __global__ void __launch_bounds__(kRaggedThreads) ragged_attention_kernel(Ragged
 
   const int g = tid / half, c = tid - g * half;
   if (g < groups) {
-    const __nv_bfloat16* vbase = a.v_cache + row0 * a.kv_stride_s + (long long)head * D + 2 * c;
+    const __nv_bfloat16* vbase = a.v_cache + row0 * a.kv_stride_s + (long long)kv_head * D + 2 * c;
     float acc0 = 0.f, acc1 = 0.f;
     for (int j = g; j < ctx; j += groups) {
       float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(vbase + (long long)j * a.kv_stride_s));
@@ -116,6 +118,7 @@ extern "C" int ab_ragged_attention(const ab::RaggedAttnArgs* a, cudaStream_t st)
   if (a->kv_stride_s % 8 != 0 || a->q_stride_t % 2 != 0) return 2;
   if (a->T <= 0) return 0;
   if (a->T > 65535 || a->max_ctx <= 0) return 5;
+  if (a->group < 1 || a->heads % a->group != 0) return 6;
   const int half = a->D / 2, groups = kRaggedThreads / half;
   if (groups < 1) return 3;
   const size_t smem = sizeof(float) * ((size_t)a->D + 8 + (size_t)groups * a->D + (size_t)a->max_ctx);

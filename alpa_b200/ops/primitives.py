@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import math
 from functools import cache
-from typing import List, Optional, Tuple
+from typing import List, NamedTuple, Optional, Tuple, Union
 
 import torch
 import torch.nn.functional as F
@@ -22,7 +22,7 @@ __all__ = [
     "swiglu_bwd", "attention", "attention_bwd", "attention_gqa_packed",
     "attention_gqa_packed_bwd", "embedding", "embedding_bwd",
     "cross_entropy", "cross_entropy_bwd", "fused_adamw_", "pipeline_marker",
-    "bmm", "moe_dispatch", "moe_combine", "moe_combine_wgrad", "moe_top2_route", "linear_fp8", "linear_decode", "decode_attention", "ragged_attention",
+    "bmm", "moe_dispatch", "moe_combine", "moe_combine_wgrad", "moe_top2_route", "linear_fp8", "linear_decode", "RMSNormArgs", "decode_attention", "decode_attention_gqa", "ragged_attention",
     "attention_cached", "attention_cached_", "quantize_mxfp8", "dequantize_mxfp8", "linear_mxfp8", "mx_pack_scale_atoms",
     "mx_unpack_scale_atoms", "pack_tiles", "unpack_tiles", "packed_nbytes",
     "dropout", "dropout_like", "dropout_keep_mask",
@@ -530,15 +530,21 @@ def _attn_unsupported(D: int, stride: int = 1) -> Optional[str]:
 
 @torch.library.custom_op("alpa_b200::attention", mutates_args=())
 def attention(q: Tensor, k: Tensor, v: Tensor, scale: float, causal: bool) -> Tuple[Tensor, Tensor]:
-    """(o [B,S,h,D], lse [B,h,S]) = softmax(q k^T * scale [+ causal mask]) v"""
+    """(o [B,S,h,D], lse [B,h,S]) = softmax(q k^T * scale [+ causal mask]) v.  A grouped q [B,S,Hkv,G,D] against k / v
+    [B,S,Hkv,D] (query head kv * G + g uses K/V head kv) gives o [B,S,Hkv,G,D] and lse [B,Hkv,G,S]."""
     if C := _kernels("attention", q, k, v, unsupported=_attn_unsupported(q.shape[-1], q.stride(-1))):
         o, lse = C.attention_fwd(q, k, v, scale, causal)
         return o, lse
+    if q.dim() == 5:
+        return _gqa_attn_ref(q, k, v, scale, causal)
     return _attn_ref(q, k, v, scale, causal)
 
 
 @attention.register_fake
 def _(q, k, v, scale, causal):
+    if q.dim() == 5:
+        B, S, Hkv, G, D = q.shape
+        return q.new_empty(B, S, Hkv, G, D), q.new_empty(B, Hkv, G, S, dtype=torch.float32)
     B, S, H, D = q.shape
     return q.new_empty(B, S, H, D), q.new_empty(B, H, S, dtype=torch.float32)
 
@@ -549,6 +555,8 @@ def attention_bwd(do: Tensor, q: Tensor, k: Tensor, v: Tensor, o: Tensor, lse: T
     if C := _kernels("attention_bwd", do, q, k, v, o, unsupported=_attn_unsupported(q.shape[-1], q.stride(-1))):
         dq, dk, dv = C.attention_bwd(do, q, k, v, o, lse, scale, causal)
         return dq, dk, dv
+    if q.dim() == 5:
+        return _gqa_attn_ref_bwd(do, q, k, v, o, lse, scale, causal)
     return _attn_ref_bwd(do, q, k, v, o, lse, scale, causal)
 
 
@@ -884,6 +892,41 @@ def decode_attention(q: Tensor, k_new: Tensor, v_new: Tensor, k_cache: Tensor, v
     return _attn_ref(q, k_cache[:, :n], v_cache[:, :n], scale, True)[0]
 
 
+def _decode_gqa_unsupported(qkv_new: Tensor) -> Optional[str]:
+    """Why the decode kernel's packed form cannot take qkv_new [B, 1, Hkv, G + 2, D], or None: it reads each head's D
+    channels and their rotary partners 16 bytes at a time from one contiguous row."""
+    D = qkv_new.shape[-1]
+    if D % 16 or D > 128:
+        return "head dim not a multiple of 16 up to 128"
+    return None if qkv_new.is_contiguous() and qkv_new.data_ptr() % 16 == 0 else "packed row not contiguous"
+
+
+def decode_attention_gqa(qkv_new: Tensor, k_cache: Tensor, v_cache: Tensor, kv_len: Tensor,
+                         position_ids: Optional[Tensor], scale: float, theta: float = 10000.0) -> Tensor:
+    """Grouped-query decode step over the packed QKV row of the new token, qkv_new [B, 1, Hkv, G + 2, D] (the QKV
+    projection's output: per K/V head its G query heads, k, v).  With `position_ids` (int64 [B, 1] on the device) the
+    query heads and k are first rotated as `rotary_packed(qkv_new, position_ids, theta, False)` rotates them, bit for
+    bit; None = no rotary.  The (rotated) k and v are appended to k/v_cache [B, S_max, Hkv, D] at row kv_len - 1
+    (kv_len: int32 device scalar, valid rows including the new one), then query head kv * G + g attends to rows
+    [0, kv_len) of K/V head kv.  One kernel launch that reads every cache row once for its whole group; one captured
+    CUDA graph serves every position.  Returns o [B, 1, Hkv * G, D]."""
+    B, _, Hkv, P, D = qkv_new.shape
+    rope = position_ids is not None
+    inv_freq = _inv_freq(D, float(theta), str(qkv_new.device)) if rope else None
+    if C := _kernels("decode_attention_gqa", qkv_new, k_cache, v_cache,
+                     unsupported=lambda: _decode_gqa_unsupported(qkv_new)):
+        pos = position_ids.to(torch.int64).reshape(B, 1).contiguous() if rope else None
+        return C.decode_attention_packed(qkv_new, k_cache, v_cache, kv_len, scale, pos, inv_freq)
+    if rope:
+        qkv_new = _rotary_ref(qkv_new, position_ids, inv_freq, False)
+    q, k, v = _gqa_split(qkv_new)
+    n = int(kv_len)
+    k_cache[:, n - 1:n] = k
+    v_cache[:, n - 1:n] = v
+    o, _ = _gqa_attn_ref(q, k_cache[:, :n], v_cache[:, :n], scale, True)
+    return o.reshape(B, 1, Hkv * (P - 2), D)
+
+
 # =================================================================================================
 # traceable attention over a KV cache (functional: returns the appended caches) -- the op `@parallelize` sees when a
 # decoder with a cache goes through the ILP / the inference pipeline (reference: examples/llm_serving/model/
@@ -931,7 +974,8 @@ def attention_cached_(q: Tensor, k_new: Tensor, v_new: Tensor, k_cache: Tensor, 
 # =================================================================================================
 def ragged_attention(q: Tensor, k_cache: Tensor, v_cache: Tensor, seq_start: Tensor, ctx_len: Tensor, scale: float,
                      max_ctx: int, alibi: Optional[Tensor] = None) -> Tensor:
-    """q: [T, h, D]; k/v_cache: [slots, h, D]; token t attends to cache rows seq_start[t] .. seq_start[t]+ctx_len[t]-1
+    """q: [T, h, D]; k/v_cache: [slots, h_kv, D] with h_kv dividing h (grouped-query attention: query head i reads
+    cache head i // (h / h_kv)); token t attends to cache rows seq_start[t] .. seq_start[t]+ctx_len[t]-1
     (ctx_len 0 = padding token -> zeros).  `max_ctx` bounds ctx_len (sizes the score buffer).  `alibi`: optional fp32
     [h] slopes, bias = slope * key position.  (reference: the external fused_mmha of opt_model_1d.py:151-178)"""
     if C := _kernels("ragged_attention", q, k_cache, v_cache):
@@ -947,8 +991,9 @@ def ragged_attention(q: Tensor, k_cache: Tensor, v_cache: Tensor, seq_start: Ten
         return torch.zeros_like(q)
     j = torch.arange(n, device=q.device)
     idx = (seq_start.long()[:, None] + j[None, :]).clamp_(max=k_cache.shape[0] - 1)          # [T, n]
-    k = k_cache[idx].float()                                                                     # [T, n, h, D]
-    v = v_cache[idx].float()
+    G = h // k_cache.shape[1]
+    k = k_cache[idx].float().repeat_interleave(G, dim=2)                                         # [T, n, h, D]
+    v = v_cache[idx].float().repeat_interleave(G, dim=2)
     s = torch.einsum("thd,tnhd->thn", q.float() * scale, k)
     if alibi is not None:
         s = s + alibi.view(1, h, 1) * j.view(1, 1, n)
@@ -1041,13 +1086,29 @@ def dropout_like(x: Tensor, p: float, seed: Tensor, stream: int = 0, training: b
 # =================================================================================================
 # fp8 weight linear (serving): w is e4m3 with one fp32 scale per output channel
 # =================================================================================================
+class RMSNormArgs(NamedTuple):
+    """The RMSNorm a serving projection applies to its input, y = x * rsqrt(mean(x^2) + eps) * gamma: passed as `ln`
+    where a LayerNorm is passed as (gamma, beta, eps)."""
+    gamma: Tensor
+    eps: float
+
+
+def norm_rows(x: Tensor, ln: Union[Tuple[Tensor, Tensor, float], RMSNormArgs]) -> Tensor:
+    """x normalised by `ln`: a LayerNorm (gamma, beta, eps) or an RMSNormArgs."""
+    if isinstance(ln, RMSNormArgs):
+        return rms_norm(x, ln.gamma, ln.eps)[0]
+    return layer_norm(x, ln[0], ln[1], ln[2])[0]
+
+
 def linear_decode(x: Tensor, w: Tensor, w_scale: Optional[Tensor], b: Optional[Tensor] = None, act: str = "none",
-                  residual: Optional[Tensor] = None, ln: Optional[Tuple[Tensor, Tensor, float]] = None) -> Tensor:
+                  residual: Optional[Tensor] = None,
+                  ln: Optional[Union[Tuple[Tensor, Tensor, float], RMSNormArgs]] = None) -> Tensor:
     """y = act(LN(x) @ W^T * w_scale + b) (+ residual) for a handful of tokens (decode): weight-streaming GEMV on
     sm_90a (the streamed fp8 / bf16 weight bytes go to the tensor cores unconverted; with fp8 weights the activations
     are quantised per token to e4m3 inside the kernel, like the prefill fp8 GEMM; no tile padding); not
     differentiable.  x: [..., K] with at most 8 rows in total.  `ln` = (gamma, beta, eps) layer-normalises x inside the
-    kernel's prologue (one launch less per projection); None = x is used as is."""
+    kernel's prologue (one launch less per projection), `ln` = RMSNormArgs(gamma, eps) RMS-normalises it there; None =
+    x is used as is."""
     rows = x.numel() // x.shape[-1]
     K = x.shape[-1]
     fp8w = w.dtype == torch.float8_e4m3fn
@@ -1060,14 +1121,18 @@ def linear_decode(x: Tensor, w: Tensor, w_scale: Optional[Tensor], b: Optional[T
             x2 = x2.contiguous()
         r2 = None if residual is None else _as2d(residual)
         if ln is not None and ln[0].dtype != torch.bfloat16:
-            x2 = layer_norm(x2, ln[0], ln[1], ln[2])[0]          # the fused prologue reads bf16 gamma / beta
+            x2 = norm_rows(x2, ln)          # the fused prologue reads bf16 gamma (/ beta)
             ln = None
         if ln is None:
             y = C.gemv_decode(x2, w, w_scale, b, r2, _ACT_IDS[act])
+        elif isinstance(ln, RMSNormArgs):
+            y = C.gemv_decode(x2, w, w_scale, b, r2, _ACT_IDS[act], ln.gamma, None, float(ln.eps), True)
         else:
             y = C.gemv_decode(x2, w, w_scale, b, r2, _ACT_IDS[act], ln[0], ln[1], float(ln[2]))
         return y.view(*x.shape[:-1], w.shape[0])
-    if ln is not None:
+    if isinstance(ln, RMSNormArgs):
+        x = _rms_ref(x, ln.gamma, ln.eps)[0]
+    elif ln is not None:
         x = F.layer_norm(x.float(), (K,), ln[0].float(), ln[1].float(), ln[2]).to(x.dtype)
     wf = w.to(torch.float32) * w_scale[:, None] if w_scale is not None else w.to(torch.float32)
     y = _act_fn(F.linear(x.float(), wf, None if b is None else b.float()), act)
@@ -1624,6 +1689,8 @@ class _FastNamespace:
         self.linear_fp8 = linear_fp8
         self.linear_decode = linear_decode
         self.decode_attention = decode_attention
+        self.decode_attention_gqa = decode_attention_gqa
+        self.norm_rows = norm_rows
         self.ragged_attention = ragged_attention
         self.linear_mxfp8 = linear_mxfp8
 

@@ -400,6 +400,8 @@ def load_params_np(cfg: OPTConfig, path: str) -> Dict[str, torch.Tensor]:
         return _load_bloom_params(cfg, ld)
     if cfg.arch == "codegen":
         return _load_codegen_params(cfg, ld)
+    if cfg.arch == "llama":
+        return _load_llama_params(cfg, path, ld)
     p: Dict[str, torch.Tensor] = {"embed_tokens": ld("decoder.embed_tokens.weight"),
                                   "embed_positions": ld("decoder.embed_positions.weight"),
                                   "final_ln.g": ld("decoder.layer_norm.weight"), "final_ln.b": ld("decoder.layer_norm.bias")}
@@ -435,6 +437,17 @@ def _load_bloom_params(cfg: OPTConfig, ld) -> Dict[str, torch.Tensor]:
         p[o + "fc1.w"], p[o + "fc1.b"] = ld(b + "mlp.dense_h_to_4h.weight"), ld(b + "mlp.dense_h_to_4h.bias")
         p[o + "fc2.w"], p[o + "fc2.b"] = ld(b + "mlp.dense_4h_to_h.weight"), ld(b + "mlp.dense_4h_to_h.bias")
     return p
+
+
+def _load_llama_params(cfg: OPTConfig, path: str, ld) -> Dict[str, torch.Tensor]:
+    """Hugging Face Llama names (`model.layers.N.self_attn.q_proj.weight`, ...; with or without the `model.` prefix)
+    through `llama_params_from_hf` into the `GPTModel(arch="llama")` layout DecoderLM takes."""
+    import os
+
+    from alpa_b200.model.gpt_model import llama_params_from_hf
+    from alpa_b200.model.opt_model import gpt_config_from_serving
+    sd = {name: ld(name) for name in os.listdir(path) if name.endswith(".weight")}
+    return llama_params_from_hf(sd, gpt_config_from_serving(cfg))
 
 
 CODEGEN_MP_NUM = 4      # the released CodeGen checkpoints interleave qkv_proj for 4-way model parallelism

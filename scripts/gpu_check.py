@@ -428,9 +428,46 @@ def sec_llama_step():
     alpa.shutdown()
 
 
+def sec_llama_decode():
+    """Grouped-query decode attention (fused rotary + cache append) at the Llama-3-8B shape (Hkv = 8, G = 4, D = 128),
+    against the multi-head kernel on the cache expanded to 32 heads, which is what serving GQA took before.  Bytes are
+    the K / V rows each kernel must read (2 * B * kv_len * heads * D * 2); the share is of 3.35 TB/s (H100 SXM data
+    sheet), for the grouped kernel's bytes.  L2 flushed before each call."""
+    Hkv, G, D, theta = 8, 4, 128, 500000.0
+    scale = D ** -0.5
+    print("llama_decode: B ctx | grouped us GB/s share | expanded-MHA us GB/s | speed-up", flush=True)
+    for B in (1, 8, 32):
+        for ctx in (1024, 4096, 16384):
+            torch.manual_seed(0)
+            qkv = torch.randn(B, 1, Hkv, G + 2, D, device="cuda", dtype=torch.bfloat16)
+            kc = torch.randn(B, ctx, Hkv, D, device="cuda", dtype=torch.bfloat16)
+            vc = torch.randn_like(kc)
+            kv_len = torch.full((1,), ctx, dtype=torch.int32, device="cuda")
+            pos = torch.full((B, 1), ctx - 1, dtype=torch.long, device="cuda")
+            t_g = median_ms(lambda: ops.fast.decode_attention_gqa(qkv, kc, vc, kv_len, pos, scale, theta), flush=True)
+            o_g = ops.fast.decode_attention_gqa(qkv, kc, vc, kv_len, pos, scale, theta)
+            # the expanded multi-head form of the same step: rotated row, K / V repeated per query head
+            rot = ops.rotary_packed(qkv, pos, theta, False)
+            q = rot[:, :, :, :G].reshape(B, 1, Hkv * G, D)
+            kn = rot[:, :, :, G:G + 1].expand(-1, -1, -1, G, -1).reshape(B, 1, Hkv * G, D).contiguous()
+            vn = rot[:, :, :, G + 1:].expand(-1, -1, -1, G, -1).reshape(B, 1, Hkv * G, D).contiguous()
+            ke = kc.repeat_interleave(G, 2)
+            ve = vc.repeat_interleave(G, 2)
+            del kc, vc
+            t_e = median_ms(lambda: ops.fast.decode_attention(q, kn, vn, ke, ve, kv_len, scale), flush=True)
+            o_e = ops.fast.decode_attention(q, kn, vn, ke, ve, kv_len, scale)
+            check(f"llama_decode B={B} ctx={ctx} grouped vs expanded", o_g.float(), o_e.float(), 2e-2, 2e-2)
+            nbytes = 2 * B * ctx * Hkv * D * 2
+            gbs_g, gbs_e = nbytes / t_g / 1e6, G * nbytes / t_e / 1e6
+            print(f"llama_decode: B={B:2d} ctx={ctx:5d} | {t_g * 1e3:8.1f} us {gbs_g:7.0f} GB/s "
+                  f"{gbs_g / 3350:5.1%} | {t_e * 1e3:8.1f} us {gbs_e:7.0f} GB/s | {t_e / t_g:4.2f}x", flush=True)
+            del ke, ve
+            torch.cuda.empty_cache()
+
+
 SECTIONS = {"gemm_bench": sec_gemm_bench, "gemm_sweep": sec_gemm_sweep, "misc": sec_misc, "attn": sec_attn,
             "attn_gqa": sec_attn_gqa, "moe": sec_moe, "fp8": sec_fp8, "gemv": sec_gemv, "ragged": sec_ragged,
-            "llama": sec_llama, "llama_step": sec_llama_step}
+            "llama": sec_llama, "llama_step": sec_llama_step, "llama_decode": sec_llama_decode}
 
 
 def card():
