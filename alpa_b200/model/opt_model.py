@@ -9,7 +9,9 @@ H100 design: a dedicated SPMD inference engine -- one process per GPU, Megatron 
 explicitly (column-parallel QKV / FC1, row-parallel out-proj / FC2, vocab-parallel embedding and LM head), the
 all-reduces on the NVSwitch (NCCL / NVLS), KV cache resident in HBM as [B, S_max, heads_local, D] per layer, the
 prompt phase on the flash-attention kernel and every decode step replayed from a CUDA graph.  Weights can be kept in
-fp8 (e4m3, per-output-channel scales) to halve the weight traffic that bounds decode.
+fp8 (e4m3, per-output-channel scales) to halve the weight traffic that bounds decode, and the KV cache in fp8
+(`kv_cache_dtype="fp8"`: e4m3 rows with one scale per token and head, `ops.Fp8KV`) to halve the cache traffic that
+bounds decode at long contexts and large batches.
 
 `arch="llama"` serves the Llama-style model of `gpt_model.GPTModel(arch="llama")` from its parameters: pre-RMSNorm
 blocks without biases, grouped-query attention with rotary embeddings, a SwiGLU MLP.  Its KV cache holds only the K/V
@@ -53,8 +55,12 @@ class OPTConfig:
     # the RMSNorm eps and ffn_dim the SwiGLU width
     num_key_value_heads: Optional[int] = None
     rope_theta: float = 10000.0
+    # bf16 | fp8: e4m3 K/V rows with one fp32 scale per (token, K/V head) (ops.Fp8KV), about half the cache bytes
+    kv_cache_dtype: str = "bf16"
 
     def __post_init__(self):
+        if self.kv_cache_dtype not in ("bf16", "fp8"):
+            raise ValueError(f"kv_cache_dtype must be 'bf16' or 'fp8', not {self.kv_cache_dtype!r}")
         if self.parallel_block is None:
             self.parallel_block = self.arch == "codegen"
         if self.tie_word_embeddings is None:
@@ -324,11 +330,37 @@ class DecoderLM:
         self.head_b = None
 
     # ------------------------------------------------------------------ cache
+    def _new_kv(self, shape):
+        if self.cfg.kv_cache_dtype == "fp8":
+            return ops.Fp8KV.zeros(shape, self.device), ops.Fp8KV.zeros(shape, self.device)
+        return (torch.zeros(shape, dtype=self.cfg.dtype, device=self.device),
+                torch.zeros(shape, dtype=self.cfg.dtype, device=self.device))
+
     def init_cache(self, batch_size: int, max_len: int):
-        """(reference: init_cache_np, opt_model.py:756) -> list of (k, v) [B, max_len, kv_heads_local, D]"""
-        shape = (batch_size, max_len, self.kv_local, self.D)
-        return [(torch.zeros(shape, dtype=self.cfg.dtype, device=self.device),
-                 torch.zeros(shape, dtype=self.cfg.dtype, device=self.device)) for _ in self.layers]
+        """(reference: init_cache_np, opt_model.py:756) -> list of (k, v) [B, max_len, kv_heads_local, D]: bf16
+        tensors, or ops.Fp8KV caches of that data shape when cfg.kv_cache_dtype is "fp8"."""
+        return [self._new_kv((batch_size, max_len, self.kv_local, self.D)) for _ in self.layers]
+
+    @staticmethod
+    def _cache_write(kc, vc, k, v, at):
+        """Write k / v [B, T, Hkv, D] into the cache: at rows at .. at + T - 1 of every sequence (`at` an int), or at
+        the slots `at` (int64 [T], B = 1) of a slot-addressed cache."""
+        slots = isinstance(at, torch.Tensor)
+        if isinstance(kc, ops.Fp8KV):
+            ops.fast.kv_cache_store(k, v, kc, vc, 0 if slots else at, at if slots else None)
+        elif not slots:
+            kc[:, at:at + k.shape[1]] = k
+            vc[:, at:at + k.shape[1]] = v
+        else:
+            kc.index_copy_(0, at, k[0].contiguous())
+            vc.index_copy_(0, at, v[0].contiguous())
+
+    @staticmethod
+    def _cache_read(kc, vc, end: int):
+        """bf16 K / V [B, end, Hkv, D] of cache rows [0, end): views of a bf16 cache, a dequantised copy of an fp8 one."""
+        if isinstance(kc, ops.Fp8KV):
+            return ops.fast.kv_cache_load(kc, end), ops.fast.kv_cache_load(vc, end)
+        return kc[:, :end], vc[:, :end]
 
     def weight_bytes(self) -> int:
         n = self.wte.numel() * 2 + (0 if self.head_w is self.wte else self.head_w.numel() * 2)
@@ -433,12 +465,12 @@ class DecoderLM:
             q, k, v = qkv[:, :, :, 0], qkv[:, :, :, 1], qkv[:, :, :, 2]
             if cfg.rotary_dim:
                 q, k = self._rotary(q, k, position_ids)
-            kc[:, cache_len:end] = k
-            vc[:, cache_len:end] = v
+            self._cache_write(kc, vc, k, v, cache_len)
+            kk, vv = self._cache_read(kc, vc, end)
             if self.alibi is None:
-                o, _ = ops.fast.attention(q if q.stride(-1) == 1 else q.contiguous(), kc[:, :end], vc[:, :end], scale, True)
+                o, _ = ops.fast.attention(q if q.stride(-1) == 1 else q.contiguous(), kk, vv, scale, True)
             else:
-                o = self._attention_alibi(q, kc[:, :end], vc[:, :end], scale, cache_len)
+                o = self._attention_alibi(q, kk, vv, scale, cache_len)
             a = l["out"](o.reshape(B, T, self.nh_local * self.D))
             if cfg.parallel_block:                  # x + attn(ln(x)) + mlp(ln(x)): one all-reduce for both branches
                 x = x + self._all_reduce(a + l["fc2"](l["fc1"](h, cfg.activation)))
@@ -466,10 +498,9 @@ class DecoderLM:
             h = ops.fast.norm_rows(x, l["ln1"])
             qkv = l["qkv"](h).view(B, T, self.kv_local, G + 2, self.D)
             qkv = ops.fast.rotary_packed(qkv, position_ids, cfg.rope_theta, False)
-            kc[:, cache_len:end] = qkv[:, :, :, G]
-            vc[:, cache_len:end] = qkv[:, :, :, G + 1]
+            self._cache_write(kc, vc, qkv[:, :, :, G], qkv[:, :, :, G + 1], cache_len)
             # the grouped Q view against the valid cache rows: causal with Sq != Sk
-            o, _ = ops.fast.attention(qkv[:, :, :, :G], kc[:, :end], vc[:, :end], scale, True)
+            o, _ = ops.fast.attention(qkv[:, :, :, :G], *self._cache_read(kc, vc, end), scale, True)
             x = x + self._all_reduce(l["out"](o.reshape(B, T, self.nh_local * self.D)))
             x = x + self._all_reduce(self._mlp_llama(l, ops.fast.norm_rows(x, l["ln2"])))
         if last_only:
@@ -540,9 +571,7 @@ class DecoderLM:
     def init_cache_1d(self, num_slots: int):
         """Slot-addressed cache: per layer (k, v) of [num_slots + 1, heads_local, D]; the last row is the scratch row
         padding tokens write to.  (reference: init_cache_np of opt_model_1d.py:457 -- a 1-D token cache)"""
-        shape = (num_slots + 1, self.kv_local, self.D)
-        return [(torch.zeros(shape, dtype=self.cfg.dtype, device=self.device),
-                 torch.zeros(shape, dtype=self.cfg.dtype, device=self.device)) for _ in self.layers]
+        return [self._new_kv((num_slots + 1, self.kv_local, self.D)) for _ in self.layers]
 
     def forward_1d(self, input_ids: torch.Tensor, position: torch.Tensor, slot: torch.Tensor, seq_start: torch.Tensor,
                    ctx_len: torch.Tensor, cache, max_ctx: int, logit_index: torch.Tensor) -> torch.Tensor:
@@ -561,8 +590,7 @@ class DecoderLM:
             for l, (kc, vc) in zip(self.layers, cache):
                 qkv = l["qkv"](ops.fast.norm_rows(x, l["ln1"])).view(1, T, self.kv_local, G + 2, self.D)
                 qkv = ops.fast.rotary_packed(qkv, position.view(1, T), cfg.rope_theta, False)[0]
-                kc.index_copy_(0, slot, qkv[:, :, G].contiguous())
-                vc.index_copy_(0, slot, qkv[:, :, G + 1].contiguous())
+                self._cache_write(kc, vc, qkv[None, :, :, G], qkv[None, :, :, G + 1], slot)
                 q = qkv[:, :, :G].reshape(T, self.nh_local, self.D)
                 o = ops.fast.ragged_attention(q, kc, vc, seq_start, ctx_len, scale, max_ctx)
                 x = x + self._all_reduce(l["out"](o.reshape(T, self.nh_local * self.D)))
@@ -575,8 +603,7 @@ class DecoderLM:
             if cfg.rotary_dim:
                 q, k = self._rotary(q[None], k[None], position.view(1, T))
                 q, k = q[0], k[0]
-            kc.index_copy_(0, slot, k.contiguous())
-            vc.index_copy_(0, slot, v.contiguous())
+            self._cache_write(kc, vc, k[None], v[None], slot)
             o = ops.fast.ragged_attention(q, kc, vc, seq_start, ctx_len, scale, max_ctx, alibi)
             a = l["out"](o.reshape(T, self.nh_local * self.D))
             if cfg.parallel_block:

@@ -328,24 +328,41 @@ std::vector<Tensor> attention_fwd(const Tensor& q, const Tensor& k, const Tensor
 
 // Attention of a ragged 1-D token batch against a slot-addressed KV cache (see ragged_attention_sm90.cu).
 Tensor ragged_attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& seq_start,
-                        const Tensor& ctx_len, double scale, int64_t max_ctx, const OptTensor& alibi) {
+                        const Tensor& ctx_len, double scale, int64_t max_ctx, const OptTensor& alibi,
+                        const OptTensor& k_scale, const OptTensor& v_scale) {
   TORCH_CHECK(q.dim() == 3 && q.stride(2) == 1 && q.scalar_type() == at::kBFloat16, "ragged_attention: q must be bf16 [T, heads, D]");
-  TORCH_CHECK(k_cache.dim() == 3 && v_cache.dim() == 3 && k_cache.scalar_type() == at::kBFloat16 &&
-              v_cache.scalar_type() == at::kBFloat16, "ragged_attention: caches must be bf16 [slots, heads, D]");
+  const bool fp8 = k_cache.scalar_type() == at::kFloat8_e4m3fn;
+  TORCH_CHECK(k_cache.dim() == 3 && v_cache.dim() == 3 && (fp8 || k_cache.scalar_type() == at::kBFloat16) &&
+              v_cache.scalar_type() == k_cache.scalar_type(),
+              "ragged_attention: caches must be bf16 or float8_e4m3fn [slots, heads, D]");
   TORCH_CHECK(k_cache.stride(2) == 1 && k_cache.stride(1) == k_cache.size(2) && v_cache.strides() == k_cache.strides() &&
               v_cache.sizes() == k_cache.sizes(), "ragged_attention: cache rows must be dense");
   TORCH_CHECK(k_cache.size(1) > 0 && q.size(1) % k_cache.size(1) == 0 && k_cache.size(2) == q.size(2),
               "ragged_attention: the cache's heads must divide q's heads (grouped-query attention), head dims equal");
   TORCH_CHECK(aligned(k_cache.data_ptr(), 16) && aligned(v_cache.data_ptr(), 16),
               "ragged_attention: cache bases must be 16-byte aligned (16-byte K loads)");
+  TORCH_CHECK(!fp8 || k_cache.size(2) % 8 == 0, "ragged_attention: an fp8 cache needs a head dim that is a multiple of 8");
   TORCH_CHECK(seq_start.scalar_type() == at::kInt && ctx_len.scalar_type() == at::kInt && seq_start.is_contiguous() &&
               ctx_len.is_contiguous() && seq_start.numel() == q.size(0) && ctx_len.numel() == q.size(0) &&
               seq_start.is_cuda() && ctx_len.is_cuda(), "ragged_attention: seq_start / ctx_len must be int32 CUDA [T]");
   c10::cuda::CUDAGuard guard(q.device());
   ab::RaggedAttnArgs a;
   a.q = bf16_ptr(q);
-  a.k_cache = bf16_ptr(k_cache);
-  a.v_cache = bf16_ptr(v_cache);
+  a.k_cache = k_cache.data_ptr();
+  a.v_cache = v_cache.data_ptr();
+  if (fp8) {
+    // scales [heads_kv, slots]: row r of cache head h at h * stride(0) + r
+    const int64_t Hkv = k_cache.size(1), slots = k_cache.size(0);
+    for (const OptTensor* t : {&k_scale, &v_scale})
+      TORCH_CHECK(t->has_value() && (*t)->defined() && (*t)->scalar_type() == at::kFloat && (*t)->dim() == 2 &&
+                      (*t)->size(0) == Hkv && (*t)->size(1) == slots && (*t)->stride(1) == 1 &&
+                      (*t)->strides() == k_scale->strides() && (*t)->device() == k_cache.device(),
+                  "ragged_attention: an fp8 cache needs fp32 scales [heads_kv, slots] with equal strides");
+    a.cache_fp8 = 1;
+    a.k_scale = k_scale->data_ptr<float>();
+    a.v_scale = v_scale->data_ptr<float>();
+    a.scale_stride_h = k_scale->stride(0);
+  }
   Tensor o = torch::empty({q.size(0), q.size(1), q.size(2)}, q.options());
   a.o = reinterpret_cast<__nv_bfloat16*>(o.data_ptr());
   a.seq_start = seq_start.data_ptr<int>();
@@ -1042,19 +1059,41 @@ void launch_decode_attention(ab::DecodeAttnArgs& a, int max_splits, const Tensor
   g_launches += 1;
 }
 
+// fp8 cache [B, S_max, Hkv, D] e4m3: its scales are fp32 [B, Hkv, S_max] (head-major, S_max contiguous).  Checks the
+// dtypes of a cache pair and, for fp8, sets the scale pointers and strides; returns whether the cache is fp8.
+bool decode_cache_dtype(ab::DecodeAttnArgs& a, const Tensor& k_cache, const Tensor& v_cache, const OptTensor& k_scale,
+                        const OptTensor& v_scale, const char* op) {
+  const bool fp8 = k_cache.scalar_type() == at::kFloat8_e4m3fn;
+  TORCH_CHECK((fp8 || k_cache.scalar_type() == at::kBFloat16) && v_cache.scalar_type() == k_cache.scalar_type(), op,
+              ": caches must be bf16 or float8_e4m3fn");
+  if (!fp8) return false;
+  for (const OptTensor* t : {&k_scale, &v_scale})
+    TORCH_CHECK(t->has_value() && (*t)->defined() && (*t)->scalar_type() == at::kFloat && (*t)->dim() == 3 &&
+                    (*t)->size(0) == k_cache.size(0) && (*t)->size(1) == k_cache.size(2) &&
+                    (*t)->size(2) == k_cache.size(1) && (*t)->stride(2) == 1 && (*t)->strides() == k_scale->strides() &&
+                    (*t)->device() == k_cache.device(),
+                op, ": an fp8 cache needs fp32 scales [B, Hkv, S_max] with equal strides, S_max contiguous");
+  a.cache_fp8 = 1;
+  a.k_scale = k_scale->data_ptr<float>();
+  a.v_scale = v_scale->data_ptr<float>();
+  a.scale_stride_b = k_scale->stride(0);
+  a.scale_stride_h = k_scale->stride(1);
+  return true;
+}
+
 // Decode-step attention, cache append fused: q / k_new / v_new [B, 1, heads, D] views, caches [B, S_max, heads, D].
 Tensor decode_attention(const Tensor& q, const Tensor& k_new, const Tensor& v_new, Tensor k_cache, Tensor v_cache,
-                        const Tensor& kv_len, double scale) {
+                        const Tensor& kv_len, double scale, const OptTensor& k_scale, const OptTensor& v_scale) {
   TORCH_CHECK(q.is_cuda() && q.dim() == 4 && q.size(1) == 1 && q.scalar_type() == at::kBFloat16 && q.stride(3) == 1,
               "decode_attention: q must be bf16 [B, 1, heads, D]");
   TORCH_CHECK(k_new.sizes() == q.sizes() && v_new.sizes() == q.sizes() && k_new.scalar_type() == at::kBFloat16 &&
               v_new.scalar_type() == at::kBFloat16 && k_new.stride(3) == 1 && v_new.stride(3) == 1 &&
               k_new.stride(0) == v_new.stride(0) && k_new.stride(2) == v_new.stride(2),
               "decode_attention: k_new / v_new must be bf16 [B, 1, heads, D] with equal strides");
-  TORCH_CHECK(k_cache.dim() == 4 && k_cache.scalar_type() == at::kBFloat16 && v_cache.scalar_type() == at::kBFloat16 &&
+  TORCH_CHECK(k_cache.dim() == 4 &&
               k_cache.sizes() == v_cache.sizes() && k_cache.strides() == v_cache.strides() && k_cache.size(0) == q.size(0) &&
               k_cache.size(2) == q.size(2) && k_cache.size(3) == q.size(3) && k_cache.stride(3) == 1 &&
-              k_cache.stride(2) == k_cache.size(3), "decode_attention: caches must be bf16 [B, S_max, heads, D], rows dense");
+              k_cache.stride(2) == k_cache.size(3), "decode_attention: caches must be [B, S_max, heads, D], rows dense");
   TORCH_CHECK(kv_len.is_cuda() && kv_len.scalar_type() == at::kInt && kv_len.numel() == 1,
               "decode_attention: kv_len must be an int32 CUDA scalar");
   TORCH_CHECK(aligned(q.data_ptr(), 16) && aligned(k_new.data_ptr(), 16) && aligned(v_new.data_ptr(), 16) &&
@@ -1062,9 +1101,10 @@ Tensor decode_attention(const Tensor& q, const Tensor& k_new, const Tensor& v_ne
               "decode_attention: q, k_new, v_new and the caches must start on 16-byte boundaries (16-byte accesses)");
   c10::cuda::CUDAGuard guard(q.device());
   ab::DecodeAttnArgs a;
+  decode_cache_dtype(a, k_cache, v_cache, k_scale, v_scale, "decode_attention");
   a.q = bf16_ptr(q); a.k_new = bf16_ptr(k_new); a.v_new = bf16_ptr(v_new);
-  a.k_cache = reinterpret_cast<__nv_bfloat16*>(k_cache.data_ptr());
-  a.v_cache = reinterpret_cast<__nv_bfloat16*>(v_cache.data_ptr());
+  a.k_cache = k_cache.data_ptr();
+  a.v_cache = v_cache.data_ptr();
   a.kv_len = kv_len.data_ptr<int>();
   a.B = (int)q.size(0); a.heads = (int)q.size(2); a.D = (int)q.size(3); a.S_max = (int)k_cache.size(1);
   a.q_stride_b = q.stride(0); a.q_stride_h = q.stride(2);
@@ -1082,16 +1122,17 @@ Tensor decode_attention(const Tensor& q, const Tensor& k_new, const Tensor& v_ne
 // K/V head), caches [B, S_max, Hkv, D]; with position_ids [B, 1] int64 and inv_freq [D / 2] fp32 the query heads and
 // the new key are rotated first (HF's rotate_half) and the rotated key is appended.  Returns o [B, 1, Hkv * G, D].
 Tensor decode_attention_packed(const Tensor& qkv, Tensor k_cache, Tensor v_cache, const Tensor& kv_len, double scale,
-                               const OptTensor& position_ids, const OptTensor& inv_freq) {
+                               const OptTensor& position_ids, const OptTensor& inv_freq, const OptTensor& k_scale,
+                               const OptTensor& v_scale) {
   TORCH_CHECK(qkv.is_cuda() && qkv.dim() == 5 && qkv.size(1) == 1 && qkv.size(3) >= 3 &&
                   qkv.scalar_type() == at::kBFloat16 && qkv.is_contiguous(),
               "decode_attention_packed: qkv_new must be contiguous bf16 [B, 1, Hkv, G + 2, D]");
   const int64_t B = qkv.size(0), Hkv = qkv.size(2), G = qkv.size(3) - 2, D = qkv.size(4);
-  TORCH_CHECK(k_cache.dim() == 4 && k_cache.scalar_type() == at::kBFloat16 && v_cache.scalar_type() == at::kBFloat16 &&
+  TORCH_CHECK(k_cache.dim() == 4 &&
               k_cache.sizes() == v_cache.sizes() && k_cache.strides() == v_cache.strides() && k_cache.size(0) == B &&
               k_cache.size(2) == Hkv && k_cache.size(3) == D && k_cache.stride(3) == 1 && k_cache.stride(2) == D &&
               k_cache.is_cuda() && k_cache.get_device() == qkv.get_device(),
-              "decode_attention_packed: caches must be bf16 [B, S_max, Hkv, D] on qkv's device, rows dense");
+              "decode_attention_packed: caches must be [B, S_max, Hkv, D] on qkv's device, rows dense");
   TORCH_CHECK(kv_len.is_cuda() && kv_len.scalar_type() == at::kInt && kv_len.numel() == 1,
               "decode_attention_packed: kv_len must be an int32 CUDA scalar");
   TORCH_CHECK(aligned(qkv.data_ptr(), 16) && aligned(k_cache.data_ptr(), 16) && aligned(v_cache.data_ptr(), 16),
@@ -1101,6 +1142,7 @@ Tensor decode_attention_packed(const Tensor& qkv, Tensor k_cache, Tensor v_cache
               "decode_attention_packed: position_ids and inv_freq go together");
   c10::cuda::CUDAGuard guard(qkv.device());
   ab::DecodeAttnArgs a;
+  decode_cache_dtype(a, k_cache, v_cache, k_scale, v_scale, "decode_attention_packed");
   if (rope) {
     TORCH_CHECK(position_ids->is_cuda() && position_ids->scalar_type() == at::kLong && position_ids->is_contiguous() &&
                     position_ids->numel() == B && position_ids->get_device() == qkv.get_device(),
@@ -1113,8 +1155,8 @@ Tensor decode_attention_packed(const Tensor& qkv, Tensor k_cache, Tensor v_cache
   }
   const __nv_bfloat16* base = bf16_ptr(qkv);
   a.q = base; a.k_new = base + G * D; a.v_new = base + (G + 1) * D;
-  a.k_cache = reinterpret_cast<__nv_bfloat16*>(k_cache.data_ptr());
-  a.v_cache = reinterpret_cast<__nv_bfloat16*>(v_cache.data_ptr());
+  a.k_cache = k_cache.data_ptr();
+  a.v_cache = v_cache.data_ptr();
   a.kv_len = kv_len.data_ptr<int>();
   a.B = (int)B; a.kv_heads = (int)Hkv; a.group = (int)G; a.heads = (int)(Hkv * G); a.D = (int)D;
   a.S_max = (int)k_cache.size(1);
@@ -1126,6 +1168,80 @@ Tensor decode_attention_packed(const Tensor& qkv, Tensor k_cache, Tensor v_cache
   a.o = reinterpret_cast<__nv_bfloat16*>(o.data_ptr());
   launch_decode_attention(a, 64, qkv);
   return o;
+}
+
+// fp8 KV cache store: k / v [B, T, H, D] bf16 views (D contiguous, each with its own strides) are quantised into rows
+// of the caches k/v_data [B, S, H, D] (or [S, H, D]) float8_e4m3fn with scales k/v_scale [B, H, S] (or [H, S]) fp32:
+// token (b, t) goes to flat row rows[b * T + t] (int64 [B * T]) or, without rows, to b * S + start + t.  `rows` is
+// read on the device only: a value outside the cache is not written (the caller's slots must lie inside it).
+void kv_cache_store(const Tensor& k, const Tensor& v, Tensor k_data, Tensor v_data, Tensor k_scale, Tensor v_scale,
+                    int64_t start, const OptTensor& rows) {
+  TORCH_CHECK(k.dim() == 4 && k.scalar_type() == at::kBFloat16 && v.scalar_type() == at::kBFloat16 &&
+                  k.sizes() == v.sizes() && k.stride(3) == 1 && v.stride(3) == 1 && k.is_cuda() &&
+                  v.device() == k.device(),
+              "kv_cache_store: k / v must be bf16 [B, T, H, D] CUDA views of one shape, D contiguous");
+  TORCH_CHECK(aligned(k.data_ptr(), 16) && aligned(v.data_ptr(), 16), "kv_cache_store: k / v must be 16-byte aligned");
+  const bool one_d = k_data.dim() == 3;
+  TORCH_CHECK((k_data.dim() == 4 || one_d) && k_data.scalar_type() == at::kFloat8_e4m3fn &&
+                  v_data.scalar_type() == at::kFloat8_e4m3fn && k_data.sizes() == v_data.sizes() &&
+                  k_data.is_contiguous() && v_data.is_contiguous() && k_data.device() == k.device() &&
+                  v_data.device() == k.device(),
+              "kv_cache_store: caches must be contiguous float8_e4m3fn [B, S, H, D] or [S, H, D] on k's device");
+  const int64_t H = k_data.size(-2), D = k_data.size(-1), S = k_data.size(-3), Bc = one_d ? 1 : k_data.size(0);
+  TORCH_CHECK(k.size(2) == H && k.size(3) == D, "kv_cache_store: heads / head dim differ from the cache's");
+  TORCH_CHECK(k_scale.scalar_type() == at::kFloat && v_scale.scalar_type() == at::kFloat &&
+                  k_scale.sizes() == v_scale.sizes() && k_scale.strides() == v_scale.strides() &&
+                  k_scale.dim() == k_data.dim() - 1 && k_scale.size(-2) == H && k_scale.size(-1) == S &&
+                  k_scale.stride(-1) == 1 && (one_d || k_scale.size(0) == Bc) && k_scale.device() == k.device() &&
+                  v_scale.device() == k.device(),
+              "kv_cache_store: scales must be fp32 [B, H, S] (or [H, S]) with S contiguous");
+  ab::KVStoreArgs a;
+  a.B = (int)k.size(0); a.T = (int)k.size(1); a.H = (int)H; a.D = (int)D; a.S = (int)S; a.start = (int)start;
+  if (rows.has_value() && rows->defined()) {
+    TORCH_CHECK(rows->scalar_type() == at::kLong && rows->is_contiguous() && rows->numel() == k.size(0) * k.size(1) &&
+                    rows->device() == k.device(),
+                "kv_cache_store: rows must be int64 [B * T] on k's device");
+    a.rows = rows->data_ptr<int64_t>();
+  } else {
+    TORCH_CHECK(k.size(0) <= Bc && start >= 0 && start + k.size(1) <= S, "kv_cache_store: rows outside the cache");
+  }
+  a.k = bf16_ptr(k); a.v = bf16_ptr(v);
+  for (int i = 0; i < 3; ++i) {
+    a.k_stride[i] = k.stride(i);
+    a.v_stride[i] = v.stride(i);
+  }
+  a.cache_rows = Bc * S;
+  a.k_data = reinterpret_cast<uint8_t*>(k_data.data_ptr());
+  a.v_data = reinterpret_cast<uint8_t*>(v_data.data_ptr());
+  a.k_scale = k_scale.data_ptr<float>();
+  a.v_scale = v_scale.data_ptr<float>();
+  a.scale_stride_b = one_d ? 0 : k_scale.stride(0);
+  a.scale_stride_h = k_scale.stride(-2);
+  c10::cuda::CUDAGuard guard(k.device());
+  AB_CHECK_RC(ab_kv_cache_store(&a, cur_stream()), "ab_kv_cache_store");
+  g_launches += 1;
+}
+
+// fp8 KV cache load: rows [0, end) of data [B, S, H, D] float8_e4m3fn (rows dense) with scale [B, H, S] fp32,
+// dequantised into a new bf16 [B, end, H, D].
+Tensor kv_cache_load(const Tensor& data, const Tensor& scale, int64_t end) {
+  TORCH_CHECK(data.dim() == 4 && data.scalar_type() == at::kFloat8_e4m3fn && data.is_cuda() && data.stride(3) == 1 &&
+                  data.stride(2) == data.size(3) && data.stride(1) == data.size(2) * data.size(3) &&
+                  aligned(data.data_ptr(), 8),
+              "kv_cache_load: data must be float8_e4m3fn [B, S, H, D] with dense rows, 8-byte aligned");
+  const int64_t B = data.size(0), S = data.size(1), H = data.size(2), D = data.size(3);
+  TORCH_CHECK(scale.scalar_type() == at::kFloat && scale.dim() == 3 && scale.size(0) == B && scale.size(1) == H &&
+                  scale.size(2) == S && scale.stride(2) == 1 && scale.device() == data.device(),
+              "kv_cache_load: scale must be fp32 [B, H, S], S contiguous");
+  TORCH_CHECK(end >= 0 && end <= S, "kv_cache_load: end outside the cache");
+  c10::cuda::CUDAGuard guard(data.device());
+  Tensor out = torch::empty({B, end, H, D}, data.options().dtype(at::kBFloat16));
+  AB_CHECK_RC(ab_kv_cache_load(reinterpret_cast<const uint8_t*>(data.data_ptr()), scale.data_ptr<float>(),
+                               reinterpret_cast<__nv_bfloat16*>(out.data_ptr()), (int)B, (int)end, (int)H, (int)D,
+                               data.stride(0), scale.stride(0), scale.stride(1), cur_stream()),
+              "ab_kv_cache_load");
+  g_launches += 1;
+  return out;
 }
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -1170,7 +1286,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("ce_stats", &ce_stats);
   m.def("ce_grad_", &ce_grad_);
   m.def("ragged_attention", &ragged_attention, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("seq_start"),
-        py::arg("ctx_len"), py::arg("scale"), py::arg("max_ctx"), py::arg("alibi") = py::none());
+        py::arg("ctx_len"), py::arg("scale"), py::arg("max_ctx"), py::arg("alibi") = py::none(),
+        py::arg("k_scale") = py::none(), py::arg("v_scale") = py::none());
   m.def("dropout", &dropout);
   m.def("embedding_fwd", &embedding_fwd);
   m.def("embedding_bwd_", &embedding_bwd_);
@@ -1191,9 +1308,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("bias") = py::none(), py::arg("residual") = py::none(), py::arg("act") = 0,
         py::arg("ln_gamma") = py::none(), py::arg("ln_beta") = py::none(), py::arg("ln_eps") = 1e-5,
         py::arg("ln_rms") = false);
-  m.def("decode_attention", &decode_attention);
+  m.def("decode_attention", &decode_attention, py::arg("q"), py::arg("k_new"), py::arg("v_new"), py::arg("k_cache"),
+        py::arg("v_cache"), py::arg("kv_len"), py::arg("scale"), py::arg("k_scale") = py::none(),
+        py::arg("v_scale") = py::none());
   m.def("decode_attention_packed", &decode_attention_packed, py::arg("qkv_new"), py::arg("k_cache"), py::arg("v_cache"),
-        py::arg("kv_len"), py::arg("scale"), py::arg("position_ids") = py::none(), py::arg("inv_freq") = py::none());
+        py::arg("kv_len"), py::arg("scale"), py::arg("position_ids") = py::none(), py::arg("inv_freq") = py::none(),
+        py::arg("k_scale") = py::none(), py::arg("v_scale") = py::none());
+  m.def("kv_cache_store", &kv_cache_store, py::arg("k"), py::arg("v"), py::arg("k_data"), py::arg("v_data"),
+        py::arg("k_scale"), py::arg("v_scale"), py::arg("start") = 0, py::arg("rows") = py::none());
+  m.def("kv_cache_load", &kv_cache_load, py::arg("data"), py::arg("scale"), py::arg("end"));
   m.def("moe_top2_route", &moe_top2_route);
   m.def("moe_dispatch_", &moe_dispatch_, py::arg("x"), py::arg("expert"), py::arg("slot"), py::arg("weight"),
         py::arg("d"), py::arg("capacity"), py::arg("peer_ptrs") = std::vector<int64_t>(), py::arg("g_off") = 0);

@@ -11,13 +11,19 @@
 // The op is a pure cache stream (2 * kv_len * D bf16 per head), so it runs on the CUDA cores; what matters is memory
 // level parallelism: every lane keeps kUnroll K rows and kUnroll V rows (16-byte pieces) in flight.
 // Because kv_len is read on the device, one captured CUDA graph serves every decode position.
+// The cache is bf16, or fp8 (e4m3 rows with one fp32 scale per row and head, kv_fp8.cuh): a lane then loads 8 bytes
+// per row, twice as many rows are in flight, and the scales multiply the dot product and the softmax weight instead
+// of every element.
 // Reference behaviour: the per-token attention + cache update of examples/llm_serving/model/opt_model.py:213-300
 // (dynamic_update_slice into the cache, then a masked attention over the whole cache).
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "kernels.h"
+#include "kv_fp8.cuh"
 #include "pdl.h"
 #include "ptx.cuh"
 
@@ -50,9 +56,13 @@ __device__ __forceinline__ int4 rope8(int4 own, int4 oth, const float2* cs, int 
 
 // GC: query heads per CTA (one K/V head's group, or a chunk of it).  Every K / V row a CTA loads is used for all of
 // its GC query heads.  ROPE: rotate the query heads and k_new first (the appended row is the rotated one).
-template <int GC, bool ROPE>
+// Cache: __nv_bfloat16, or __nv_fp8_e4m3 with per-row scales (the appended row is quantised here).
+template <int GC, bool ROPE, typename Cache>
 __global__ void __launch_bounds__(kDecWarps * 32) decode_attention_kernel(const DecodeAttnArgs a) {
-  constexpr int kU = GC <= 2 ? kDecUnroll : 2;  // K / V rows in flight per lane: registers go to the GC queries
+  constexpr bool F8 = std::is_same_v<Cache, __nv_fp8_e4m3>;
+  // K / V rows in flight per lane: registers go to the GC queries; an fp8 row piece (8 bytes) needs half the registers
+  constexpr int kU = (GC <= 2 ? kDecUnroll : 2) * (F8 ? 2 : 1);
+  using Piece = std::conditional_t<F8, uint2, int4>;           // one lane's 8 channels of a cache row
   __shared__ float sm_m[kDecHalves], sm_l[kDecHalves];
   __shared__ float sm_acc[kDecHalves][128];
   __shared__ float2 sm_cs[ROPE ? 64 : 1];
@@ -85,11 +95,38 @@ __global__ void __launch_bounds__(kDecWarps * 32) decode_attention_kernel(const 
   const __nv_bfloat16* kn = a.k_new + (long long)b * a.new_stride_b + (long long)head * a.new_stride_h + l16 * 8;
   const __nv_bfloat16* vn = a.v_new + (long long)b * a.new_stride_b + (long long)head * a.new_stride_h + l16 * 8;
   const long long cache_off = (long long)b * a.cache_stride_b + (long long)head * D + l16 * 8;
-  const __nv_bfloat16* kc = a.k_cache + cache_off;
-  const __nv_bfloat16* vc = a.v_cache + cache_off;
+  Cache* const k_cache = static_cast<Cache*>(a.k_cache);
+  Cache* const v_cache = static_cast<Cache*>(a.v_cache);
+  const Cache* kc = k_cache + cache_off;
+  const Cache* vc = v_cache + cache_off;
   int4 krot = make_int4(0, 0, 0, 0);                            // ROPE: the rotated new key (this lane's 8 channels)
   if constexpr (ROPE) {
     if (live) krot = rope8(*reinterpret_cast<const int4*>(kn), *reinterpret_cast<const int4*>(kn + poff), sm_cs, l16 * 8, half);
+  }
+  // F8: the new row quantised (amax over the half-warp's D channels); every CTA whose key range holds it attends to
+  // these values, the same ones it appends
+  const float* ks = nullptr;
+  const float* vs = nullptr;
+  Piece knew{}, vnew{};
+  float ks_new = 0.f, vs_new = 0.f;
+  if constexpr (F8) {
+    const long long sc_off = (long long)b * a.scale_stride_b + (long long)head * a.scale_stride_h;
+    ks = a.k_scale + sc_off;
+    vs = a.v_scale + sc_off;
+    const int4 zero = make_int4(0, 0, 0, 0);
+    const int4 kraw = ROPE ? krot : live ? *reinterpret_cast<const int4*>(kn) : zero;
+    const int4 vraw = live ? *reinterpret_cast<const int4*>(vn) : zero;
+    float kf[8], vf[8];
+    float kam = kv_bf16_unpack8(kraw, kf), vam = kv_bf16_unpack8(vraw, vf);
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) {
+      kam = fmaxf(kam, __shfl_xor_sync(0xffffffffu, kam, o));
+      vam = fmaxf(vam, __shfl_xor_sync(0xffffffffu, vam, o));
+    }
+    ks_new = kv_fp8_scale(kam);
+    vs_new = kv_fp8_scale(vam);
+    knew = kv_fp8_quant8(kf, ks_new);
+    vnew = kv_fp8_quant8(vf, vs_new);
   }
 
   float qf[GC][8];
@@ -115,9 +152,18 @@ __global__ void __launch_bounds__(kDecWarps * 32) decode_attention_kernel(const 
   const int per = ((ctx + splits - 1) / splits + kDecHalves - 1) / kDecHalves * kDecHalves;
   const int k_begin = min(split * per, ctx), k_end = min(k_begin + per, ctx);
   if (split == 0 && hw == 0 && live && last >= 0 && g0 == 0) {  // cache append (once per K/V head)
-    *reinterpret_cast<int4*>(a.k_cache + cache_off + (long long)last * a.cache_stride_s) =
-        ROPE ? krot : *reinterpret_cast<const int4*>(kn);
-    *reinterpret_cast<int4*>(a.v_cache + cache_off + (long long)last * a.cache_stride_s) = *reinterpret_cast<const int4*>(vn);
+    if constexpr (F8) {
+      *reinterpret_cast<uint2*>(k_cache + cache_off + (long long)last * a.cache_stride_s) = knew;
+      *reinterpret_cast<uint2*>(v_cache + cache_off + (long long)last * a.cache_stride_s) = vnew;
+      if (l16 == 0) {
+        a.k_scale[(long long)b * a.scale_stride_b + (long long)head * a.scale_stride_h + last] = ks_new;
+        a.v_scale[(long long)b * a.scale_stride_b + (long long)head * a.scale_stride_h + last] = vs_new;
+      }
+    } else {
+      *reinterpret_cast<int4*>(k_cache + cache_off + (long long)last * a.cache_stride_s) =
+          ROPE ? krot : *reinterpret_cast<const int4*>(kn);
+      *reinterpret_cast<int4*>(v_cache + cache_off + (long long)last * a.cache_stride_s) = *reinterpret_cast<const int4*>(vn);
+    }
   }
 
   float m[GC], l[GC], acc[GC][8];
@@ -132,40 +178,74 @@ __global__ void __launch_bounds__(kDecWarps * 32) decode_attention_kernel(const 
   // the trip count is uniform over the CTA (the shuffles below use the full mask)
   for (int base = k_begin; base < k_end; base += kDecHalves * kU) {
     const int j0 = base + hw;
-    int4 kv[kU], vv[kU];
+    Piece kv[kU], vv[kU];
+    float ksc[F8 ? kU : 1], vsc[F8 ? kU : 1];                    // F8: the rows' scales
 #pragma unroll
     for (int u = 0; u < kU; ++u) {
       const int j = j0 + u * kDecHalves;
-      kv[u] = make_int4(0, 0, 0, 0);
-      vv[u] = make_int4(0, 0, 0, 0);
-      if (live && j < k_end) {
-        // the row written above is read from its source: it is not yet visible through the non-coherent path
-        if constexpr (ROPE) {
-          kv[u] = (j == last) ? krot : ld_nc_v4(kc + (long long)j * a.cache_stride_s);
-        } else {
-          const __nv_bfloat16* kp = (j == last) ? kn : kc + (long long)j * a.cache_stride_s;
-          kv[u] = ld_nc_v4(kp);
+      if constexpr (F8) {
+        kv[u] = make_uint2(0, 0);
+        vv[u] = make_uint2(0, 0);
+        ksc[u] = vsc[u] = 0.f;
+        if (live && j < k_end) {
+          if (j == last) {
+            kv[u] = knew;
+            vv[u] = vnew;
+            ksc[u] = ks_new;
+            vsc[u] = vs_new;
+          } else {
+            kv[u] = ld_nc_v2(kc + (long long)j * a.cache_stride_s);
+            vv[u] = ld_nc_v2(vc + (long long)j * a.cache_stride_s);
+            ksc[u] = __ldg(ks + j);
+            vsc[u] = __ldg(vs + j);
+          }
         }
-        const __nv_bfloat16* vp = (j == last) ? vn : vc + (long long)j * a.cache_stride_s;
-        vv[u] = ld_nc_v4(vp);
+      } else {
+        kv[u] = make_int4(0, 0, 0, 0);
+        vv[u] = make_int4(0, 0, 0, 0);
+        if (live && j < k_end) {
+          // the row written above is read from its source: it is not yet visible through the non-coherent path
+          if constexpr (ROPE) {
+            kv[u] = (j == last) ? krot : ld_nc_v4(kc + (long long)j * a.cache_stride_s);
+          } else {
+            const __nv_bfloat16* kp = (j == last) ? kn : kc + (long long)j * a.cache_stride_s;
+            kv[u] = ld_nc_v4(kp);
+          }
+          const __nv_bfloat16* vp = (j == last) ? vn : vc + (long long)j * a.cache_stride_s;
+          vv[u] = ld_nc_v4(vp);
+        }
       }
     }
     float s[GC][kU];
 #pragma unroll
     for (int u = 0; u < kU; ++u) {
-      const uint32_t* ku = reinterpret_cast<const uint32_t*>(&kv[u]);
+      if constexpr (F8) {
+        float kf[8];
+        kv_fp8_unpack8(kv[u], kf);
 #pragma unroll
-      for (int g = 0; g < GC; ++g) {
-        float d = 0.f;
+        for (int g = 0; g < GC; ++g) {
+          float d = 0.f;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float2 f = unpack_bf16x2(ku[i]);
-          d = fmaf(f.x, qf[g][2 * i], d);
-          d = fmaf(f.y, qf[g][2 * i + 1], d);
+          for (int i = 0; i < 8; ++i) d = fmaf(kf[i], qf[g][i], d);
+#pragma unroll
+          for (int o = 8; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+          s[g][u] = (j0 + u * kDecHalves < k_end) ? d * ksc[u] : -INFINITY;   // score = s_k * dot(q, k8)
         }
+      } else {
+        const uint32_t* ku = reinterpret_cast<const uint32_t*>(&kv[u]);
 #pragma unroll
-        for (int o = 8; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
-        s[g][u] = (j0 + u * kDecHalves < k_end) ? d : -INFINITY;
+        for (int g = 0; g < GC; ++g) {
+          float d = 0.f;
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const float2 f = unpack_bf16x2(ku[i]);
+            d = fmaf(f.x, qf[g][2 * i], d);
+            d = fmaf(f.y, qf[g][2 * i + 1], d);
+          }
+#pragma unroll
+          for (int o = 8; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+          s[g][u] = (j0 + u * kDecHalves < k_end) ? d : -INFINITY;
+        }
       }
     }
 #pragma unroll
@@ -181,16 +261,29 @@ __global__ void __launch_bounds__(kDecWarps * 32) decode_attention_kernel(const 
     }
 #pragma unroll
     for (int u = 0; u < kU; ++u) {
-      const uint32_t* vu = reinterpret_cast<const uint32_t*>(&vv[u]);
+      if constexpr (F8) {
+        float vf[8];
+        kv_fp8_unpack8(vv[u], vf);
 #pragma unroll
-      for (int g = 0; g < GC; ++g) {
-        const float p = ex2_approx(s[g][u] - m[g]);
-        l[g] += p;
+        for (int g = 0; g < GC; ++g) {
+          const float p = ex2_approx(s[g][u] - m[g]);
+          l[g] += p;
+          const float pv = p * vsc[u];                          // acc += (p * s_v) * v8
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float2 f = unpack_bf16x2(vu[i]);
-          acc[g][2 * i] = fmaf(p, f.x, acc[g][2 * i]);
-          acc[g][2 * i + 1] = fmaf(p, f.y, acc[g][2 * i + 1]);
+          for (int i = 0; i < 8; ++i) acc[g][i] = fmaf(pv, vf[i], acc[g][i]);
+        }
+      } else {
+        const uint32_t* vu = reinterpret_cast<const uint32_t*>(&vv[u]);
+#pragma unroll
+        for (int g = 0; g < GC; ++g) {
+          const float p = ex2_approx(s[g][u] - m[g]);
+          l[g] += p;
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const float2 f = unpack_bf16x2(vu[i]);
+            acc[g][2 * i] = fmaf(p, f.x, acc[g][2 * i]);
+            acc[g][2 * i + 1] = fmaf(p, f.y, acc[g][2 * i + 1]);
+          }
         }
       }
     }
@@ -287,10 +380,15 @@ __global__ void __launch_bounds__(kDecWarps * 32) decode_attention_kernel(const 
 // query heads per CTA: the whole group up to 8 (register budget), else chunks of 8 that each re-read the rows
 static int decode_chunk(int group) { return group == 1 ? 1 : group == 2 ? 2 : group <= 4 ? 4 : 8; }
 
+template <int GC, typename Cache>
+static cudaError_t decode_launch(const DecodeAttnArgs& a, dim3 grid, cudaStream_t st) {
+  if (a.pos != nullptr) return launch_pdl(decode_attention_kernel<GC, true, Cache>, grid, dim3(kDecWarps * 32), 0, st, a);
+  return launch_pdl(decode_attention_kernel<GC, false, Cache>, grid, dim3(kDecWarps * 32), 0, st, a);
+}
+
 template <int GC>
 static cudaError_t decode_launch(const DecodeAttnArgs& a, dim3 grid, cudaStream_t st) {
-  if (a.pos != nullptr) return launch_pdl(decode_attention_kernel<GC, true>, grid, dim3(kDecWarps * 32), 0, st, a);
-  return launch_pdl(decode_attention_kernel<GC, false>, grid, dim3(kDecWarps * 32), 0, st, a);
+  return a.cache_fp8 ? decode_launch<GC, __nv_fp8_e4m3>(a, grid, st) : decode_launch<GC, __nv_bfloat16>(a, grid, st);
 }
 
 }  // namespace ab
@@ -312,6 +410,7 @@ extern "C" int ab_decode_attention(const ab::DecodeAttnArgs* a, cudaStream_t st)
   if (a->splits > 1 && (a->ws == nullptr || a->counters == nullptr)) return 4;
   if (a->group < 1 || a->kv_heads < 1 || a->heads != a->kv_heads * a->group) return 5;
   if ((a->pos == nullptr) != (a->inv_freq == nullptr) || (a->pos != nullptr && a->D % 16 != 0)) return 6;
+  if (a->cache_fp8 && (a->k_scale == nullptr || a->v_scale == nullptr)) return 7;
   const dim3 grid(ab_decode_attention_rows(a), a->B, a->splits);
   cudaError_t e;
   switch (decode_chunk(a->group)) {

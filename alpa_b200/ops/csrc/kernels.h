@@ -111,8 +111,8 @@ struct AttnBwdArgs {
 // Ragged 1-D token batch over a slot-addressed KV cache (serving with iteration-level batching).
 struct RaggedAttnArgs {
   const __nv_bfloat16* q = nullptr;        // [T, heads, D], strides in elements, D contiguous
-  const __nv_bfloat16* k_cache = nullptr;  // [slots, heads, D], heads*D contiguous inside a row
-  const __nv_bfloat16* v_cache = nullptr;
+  const void* k_cache = nullptr;           // [slots, heads, D] bf16 or e4m3 (cache_fp8), heads*D contiguous in a row
+  const void* v_cache = nullptr;
   __nv_bfloat16* o = nullptr;              // [T, heads, D]
   const int* seq_start = nullptr;          // [T] first cache row of the token's sequence
   const int* ctx_len = nullptr;            // [T] rows attended (0 = padding token)
@@ -121,6 +121,11 @@ struct RaggedAttnArgs {
   long long q_stride_t = 0, q_stride_h = 0, o_stride_t = 0, kv_stride_s = 0;
   float scale = 1.f;
   int group = 1;  // grouped-query attention: query head h reads cache head h / group of a [slots, heads / group, D] cache
+  // fp8 cache (kv_fp8.cuh): e4m3 rows, the scale of (row r, cache head h) at k/v_scale[h * scale_stride_h + r]
+  int cache_fp8 = 0;
+  const float* k_scale = nullptr;
+  const float* v_scale = nullptr;
+  long long scale_stride_h = 0;
 };
 
 // Decode-step attention with fused KV-cache append (decode_attention_sm90.cu).  Grouped-query attention: query head
@@ -130,8 +135,8 @@ struct DecodeAttnArgs {
   const __nv_bfloat16* q = nullptr;        // [B, kv_heads, group, D] view, D contiguous
   const __nv_bfloat16* k_new = nullptr;    // [B, kv_heads, D] views with one stride pair
   const __nv_bfloat16* v_new = nullptr;
-  __nv_bfloat16* k_cache = nullptr;        // [B, S_max, kv_heads, D], kv_heads*D dense inside a row
-  __nv_bfloat16* v_cache = nullptr;
+  void* k_cache = nullptr;                 // [B, S_max, kv_heads, D] bf16 or e4m3 (cache_fp8), kv_heads*D dense in a row
+  void* v_cache = nullptr;
   __nv_bfloat16* o = nullptr;              // [B, heads, D] contiguous, heads = kv_heads * group
   const int* kv_len = nullptr;             // device scalar: valid rows including the new one
   float* ws = nullptr;                     // [B, rows, splits, chunk, D + 2] fp32 partials (splits > 1)
@@ -145,6 +150,30 @@ struct DecodeAttnArgs {
   // pos [B] int64 positions, inv_freq [D / 2] fp32; both null = none
   const int64_t* pos = nullptr;
   const float* inv_freq = nullptr;
+  // fp8 cache (kv_fp8.cuh): e4m3 rows, the scale of (sequence b, K/V head h, row s) at
+  // k/v_scale[b * scale_stride_b + h * scale_stride_h + s]; the appended row is quantised in the kernel
+  int cache_fp8 = 0;
+  float* k_scale = nullptr;
+  float* v_scale = nullptr;
+  long long scale_stride_b = 0, scale_stride_h = 0;
+};
+
+// Quantising store of bf16 K / V rows into an fp8 cache (kv_cache_sm90.cu).  Source token (b, t) of head h is at
+// k + b * k_stride[0] + t * k_stride[1] + h * k_stride[2] (v with v_stride; D contiguous); it goes to cache row
+// rows[b * T + t], or b * S + start + t when rows is null.  Cache row r of head h: data at (r * H + h) * D, scale at
+// (r / S) * scale_stride_b + h * scale_stride_h + r % S.  A row outside [0, cache_rows) is not written.
+struct KVStoreArgs {
+  const __nv_bfloat16* k = nullptr;
+  const __nv_bfloat16* v = nullptr;
+  long long k_stride[3] = {0, 0, 0}, v_stride[3] = {0, 0, 0};
+  uint8_t* k_data = nullptr;
+  uint8_t* v_data = nullptr;
+  float* k_scale = nullptr;
+  float* v_scale = nullptr;
+  long long scale_stride_b = 0, scale_stride_h = 0;
+  const int64_t* rows = nullptr;
+  int B = 0, T = 0, H = 0, D = 0, S = 0, start = 0;
+  long long cache_rows = 0;
 };
 
 // Sharding-invariant counter-based dropout (dropout_sm90.cu)
@@ -198,6 +227,10 @@ int ab_ragged_attention(const ab::RaggedAttnArgs* a, cudaStream_t st);
 int ab_decode_attention(const ab::DecodeAttnArgs* a, cudaStream_t st);
 int ab_decode_attention_rows(const ab::DecodeAttnArgs* a);  // CTA rows per sequence (kv_heads * group chunks)
 int ab_decode_attention_chunk(const ab::DecodeAttnArgs* a);  // query heads per CTA (partials per row and split)
+int ab_kv_cache_store(const ab::KVStoreArgs* a, cudaStream_t st);
+// out [B, end, H, D] bf16 = rows [0, end) of an fp8 cache [B, S, H, D] (data_stride_b = S * H * D), dequantised
+int ab_kv_cache_load(const uint8_t* data, const float* scale, __nv_bfloat16* out, int B, int end, int H, int D,
+                     long long data_stride_b, long long scale_stride_b, long long scale_stride_h, cudaStream_t st);
 int ab_dropout(const ab::DropoutArgs* a, int is_bf16, cudaStream_t st);
 int ab_rs_reduce(const __nv_bfloat16* staging, const uint32_t* flags, uint32_t expected, __nv_bfloat16* out,
                  const __nv_bfloat16* bias, const __nv_bfloat16* residual, int rows, int N, int tp,

@@ -225,6 +225,11 @@ __device__ __forceinline__ int4 ld_nc_v4(const void* p) {
                : "l"(p));
   return r;
 }
+__device__ __forceinline__ uint2 ld_nc_v2(const void* p) {
+  uint2 r;
+  asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];\n" : "=r"(r.x), "=r"(r.y) : "l"(p));
+  return r;
+}
 __device__ __forceinline__ int4 ld_volatile_v4(const void* p) {
   int4 r;
   asm volatile("ld.volatile.global.v4.s32 {%0,%1,%2,%3}, [%4];\n"

@@ -10,11 +10,16 @@
 //   pass 1  thread-per-key dot products with 16-byte K loads -> scores in shared memory, block max / sum
 //   pass 2  thread-per-channel-pair accumulation of P*V with coalesced 4-byte V loads, key range split over groups
 // The op is bandwidth bound (it streams the sequence's K and V once per query token), so it stays on the CUDA cores.
+// The cache is bf16, or fp8 (e4m3 rows with one fp32 scale per row and cache head, kv_fp8.cuh): 8-byte K loads in
+// pass 1, 2-byte V loads in pass 2, and the scales multiply the dot product and the softmax weight.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "kernels.h"
+#include "kv_fp8.cuh"
 
 namespace ab {
 
@@ -31,7 +36,9 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+template <typename Cache>
 __global__ void __launch_bounds__(kRaggedThreads) ragged_attention_kernel(RaggedAttnArgs a) {
+  constexpr bool F8 = std::is_same_v<Cache, __nv_fp8_e4m3>;
   extern __shared__ __align__(16) float smem[];
   const int head = blockIdx.x, t = blockIdx.y, tid = threadIdx.x;
   const int D = a.D;
@@ -55,19 +62,32 @@ __global__ void __launch_bounds__(kRaggedThreads) ragged_attention_kernel(Ragged
 
   const float slope = a.alibi ? a.alibi[head] : 0.f;
   const int kv_head = head / a.group;
-  const __nv_bfloat16* kbase = a.k_cache + row0 * a.kv_stride_s + (long long)kv_head * D;
+  const Cache* kbase = static_cast<const Cache*>(a.k_cache) + row0 * a.kv_stride_s + (long long)kv_head * D;
+  const float* ks = F8 ? a.k_scale + kv_head * a.scale_stride_h + row0 : nullptr;
+  const float* vs = F8 ? a.v_scale + kv_head * a.scale_stride_h + row0 : nullptr;
   float lmax = -INFINITY;
   for (int j = tid; j < ctx; j += kRaggedThreads) {
-    const int4* kr = reinterpret_cast<const int4*>(kbase + (long long)j * a.kv_stride_s);
     float s = 0.f;
-    for (int c = 0; c < D / 8; ++c) {
-      int4 pk = __ldg(kr + c);
-      const __nv_bfloat162* k2 = reinterpret_cast<const __nv_bfloat162*>(&pk);
+    if constexpr (F8) {
+      const uint2* kr = reinterpret_cast<const uint2*>(kbase + (long long)j * a.kv_stride_s);
+      for (int c = 0; c < D / 8; ++c) {
+        float f[8];
+        kv_fp8_unpack8(__ldg(kr + c), f);
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        float2 f = __bfloat1622float2(k2[e]);
-        s = fmaf(f.x, qs[c * 8 + 2 * e], s);
-        s = fmaf(f.y, qs[c * 8 + 2 * e + 1], s);
+        for (int e = 0; e < 8; ++e) s = fmaf(f[e], qs[c * 8 + e], s);
+      }
+      s *= __ldg(ks + j);                                       // score = s_k * dot(q, k8)
+    } else {
+      const int4* kr = reinterpret_cast<const int4*>(kbase + (long long)j * a.kv_stride_s);
+      for (int c = 0; c < D / 8; ++c) {
+        int4 pk = __ldg(kr + c);
+        const __nv_bfloat162* k2 = reinterpret_cast<const __nv_bfloat162*>(&pk);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          float2 f = __bfloat1622float2(k2[e]);
+          s = fmaf(f.x, qs[c * 8 + 2 * e], s);
+          s = fmaf(f.y, qs[c * 8 + 2 * e + 1], s);
+        }
       }
     }
     s += slope * (float)j;
@@ -91,11 +111,17 @@ __global__ void __launch_bounds__(kRaggedThreads) ragged_attention_kernel(Ragged
 
   const int g = tid / half, c = tid - g * half;
   if (g < groups) {
-    const __nv_bfloat16* vbase = a.v_cache + row0 * a.kv_stride_s + (long long)kv_head * D + 2 * c;
+    const Cache* vbase = static_cast<const Cache*>(a.v_cache) + row0 * a.kv_stride_s + (long long)kv_head * D + 2 * c;
     float acc0 = 0.f, acc1 = 0.f;
     for (int j = g; j < ctx; j += groups) {
-      float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(vbase + (long long)j * a.kv_stride_s));
-      const float p = sc[j];
+      float2 f;
+      float p = sc[j];
+      if constexpr (F8) {
+        f = kv_fp8_unpack2(*reinterpret_cast<const uint16_t*>(vbase + (long long)j * a.kv_stride_s));
+        p *= __ldg(vs + j);                                     // acc += (p * s_v) * v8
+      } else {
+        f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(vbase + (long long)j * a.kv_stride_s));
+      }
       acc0 = fmaf(p, f.x, acc0);
       acc1 = fmaf(p, f.y, acc1);
     }
@@ -123,12 +149,14 @@ extern "C" int ab_ragged_attention(const ab::RaggedAttnArgs* a, cudaStream_t st)
   if (groups < 1) return 3;
   const size_t smem = sizeof(float) * ((size_t)a->D + 8 + (size_t)groups * a->D + (size_t)a->max_ctx);
   if (smem > 200 * 1024) return 4;
+  if (a->cache_fp8 && (a->k_scale == nullptr || a->v_scale == nullptr)) return 7;
+  auto kernel = a->cache_fp8 ? ragged_attention_kernel<__nv_fp8_e4m3> : ragged_attention_kernel<__nv_bfloat16>;
   if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(ragged_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return 100 + (int)e;
   }
   dim3 grid(a->heads, a->T);
-  ragged_attention_kernel<<<grid, kRaggedThreads, smem, st>>>(*a);
+  kernel<<<grid, kRaggedThreads, smem, st>>>(*a);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : 100 + (int)e;
 }

@@ -23,6 +23,7 @@ __all__ = [
     "attention_gqa_packed_bwd", "embedding", "embedding_bwd",
     "cross_entropy", "cross_entropy_bwd", "fused_adamw_", "pipeline_marker",
     "bmm", "moe_dispatch", "moe_combine", "moe_combine_wgrad", "moe_top2_route", "linear_fp8", "linear_decode", "RMSNormArgs", "decode_attention", "decode_attention_gqa", "ragged_attention",
+    "Fp8KV", "kv_cache_store", "kv_cache_load", "kv_cache_nbytes",
     "attention_cached", "attention_cached_", "quantize_mxfp8", "dequantize_mxfp8", "linear_mxfp8", "mx_pack_scale_atoms",
     "mx_unpack_scale_atoms", "pack_tiles", "unpack_tiles", "packed_nbytes",
     "dropout", "dropout_like", "dropout_keep_mask",
@@ -872,6 +873,142 @@ embedding.register_autograd(_emb_bwd, setup_context=_emb_setup)
 
 
 # =================================================================================================
+# fp8 KV cache (serving): e4m3 rows with one fp32 scale per (token, K/V head)
+# =================================================================================================
+class Fp8KV:
+    """One K or V cache in fp8: `data` e4m3 [B, S, Hkv, D] with `scale` fp32 [B, Hkv, S], or the slot-addressed
+    `data` [slots, Hkv, D] with `scale` [Hkv, slots].  A row x of D bf16 values is stored as
+        s = max(amax(|x|), 1e-8) / 448,   q = e4m3_rne(x / s)    (both divisions correctly rounded)
+    and reads back as float(q) * s.  The scales are head-major so that the consecutive keys a decode CTA reads share
+    their sectors.  The serving ops (decode / ragged attention, `kv_cache_store`, `kv_cache_load`) take an Fp8KV where
+    they take a bf16 cache tensor; the batch slicing and the `index_select` / `copy_` reordering that generation
+    applies to cache tensors work on it too (4-D caches), moving data and scales together."""
+    __slots__ = ("data", "scale")
+
+    def __init__(self, data: Tensor, scale: Tensor):
+        self.data, self.scale = data, scale
+
+    @classmethod
+    def zeros(cls, shape, device) -> "Fp8KV":
+        """An all-zero cache of data shape [B, S, Hkv, D] or [slots, Hkv, D]."""
+        *lead, S, H, _ = shape
+        return cls(torch.zeros(shape, dtype=torch.float8_e4m3fn, device=device),
+                   torch.zeros(*lead, H, S, dtype=torch.float32, device=device))
+
+    def _batched(self):
+        if self.data.dim() != 4:
+            raise TypeError("batch indexing needs a [B, S, Hkv, D] cache")
+
+    def __getitem__(self, idx) -> "Fp8KV":
+        self._batched()
+        if not isinstance(idx, slice):
+            raise TypeError("Fp8KV supports slicing along the batch only")
+        return Fp8KV(self.data[idx], self.scale[idx])
+
+    def index_select(self, dim: int, index: Tensor) -> "Fp8KV":
+        self._batched()
+        if dim != 0:
+            raise ValueError("Fp8KV reorders along the batch (dim 0) only")
+        return Fp8KV(self.data.view(torch.uint8).index_select(0, index).view(torch.float8_e4m3fn),
+                     self.scale.index_select(0, index))
+
+    def copy_(self, other: "Fp8KV") -> "Fp8KV":
+        self.data.view(torch.uint8).copy_(other.data.view(torch.uint8))
+        self.scale.copy_(other.scale)
+        return self
+
+    def nbytes(self) -> int:
+        return self.data.numel() + self.scale.numel() * 4
+
+    def values(self, end: Optional[int] = None) -> Tensor:
+        """The fp32 values float(q) * s ([B, end, Hkv, D] of rows [0, end), or [slots, Hkv, D])."""
+        if self.data.dim() == 3:
+            return self.data.float() * self.scale.t()[..., None]
+        return self.data[:, :end].float() * self.scale[:, :, :end].transpose(1, 2)[..., None]
+
+
+_KV_DTYPES = (torch.bfloat16, torch.float8_e4m3fn)
+
+
+def kv_cache_nbytes(cache) -> int:
+    """Bytes held by a model's KV cache: a list of (k, v) bf16 tensors or Fp8KV pairs."""
+    return sum(t.nbytes() if isinstance(t, Fp8KV) else t.numel() * t.element_size() for kv in cache for t in kv)
+
+
+def _kv_quant_ref(x: Tensor) -> Tuple[Tensor, Tensor]:
+    """(q e4m3 [..., D], s fp32 [...]) of rows x [..., D] in the Fp8KV format.  Both divisions are tensor by tensor:
+    PyTorch divides by a Python scalar as a multiply by its reciprocal on CUDA, which is not correctly rounded."""
+    xf = x.float()
+    amax = xf.abs().amax(-1).clamp(min=1e-8)
+    s = amax / torch.full_like(amax, 448.0)
+    return (xf / s[..., None]).to(torch.float8_e4m3fn), s
+
+
+def _kv_store_ref(k: Tensor, v: Tensor, k_cache: Fp8KV, v_cache: Fp8KV, start: int, rows: Optional[Tensor]):
+    B, T, H, D = k.shape
+    for x, c in ((k, k_cache), (v, v_cache)):
+        q, sc = _kv_quant_ref(x)
+        q8 = q.view(torch.uint8)
+        if rows is None:
+            c.data.view(torch.uint8)[:B, start:start + T] = q8
+            c.scale[:B, :, start:start + T] = sc.transpose(1, 2)
+        else:
+            c.data.view(torch.uint8)[rows] = q8.reshape(B * T, H, D)
+            c.scale[:, rows] = sc.reshape(B * T, H).t()
+
+
+def _kv_store_unsupported(k: Tensor, v: Tensor) -> Optional[str]:
+    """Why the store kernel (one warp per row, 16-byte loads of 8 channels) cannot take k / v, or None."""
+    D = k.shape[-1]
+    if D % 8 or D > 256:
+        return "head dim not a multiple of 8 up to 256"
+    for x in (k, v):
+        if x.stride(-1) != 1 or any(st % 8 for st in x.stride()[:-1]) or x.data_ptr() % 16:
+            return "K / V rows not 16-byte aligned"
+    return None
+
+
+def kv_cache_store(k: Tensor, v: Tensor, k_cache: Fp8KV, v_cache: Fp8KV, start: int = 0,
+                   rows: Optional[Tensor] = None) -> None:
+    """Quantise bf16 K / V rows into fp8 caches.  k / v: [B, T, Hkv, D] views, each with its own strides (the packed
+    QKV projection's K and V slots, or a rotated K next to the V slot, are fine).  For [B, S, Hkv, D] caches token
+    (b, t) goes to row start + t of sequence b; for slot-addressed [slots, Hkv, D] caches `rows` (int64 [B * T]) gives
+    each token's slot.  The slots must lie inside the cache: the kernel reads them on the device only and writes
+    nothing for a slot outside it."""
+    if (rows is None) != (k_cache.data.dim() == 4):
+        raise ValueError("kv_cache_store: [B, S, Hkv, D] caches take `start`, slot-addressed caches take `rows`")
+    if C := _kernels("kv_cache_store", k, v, k_cache.data, v_cache.data, dtypes=_KV_DTYPES,
+                     unsupported=lambda: _kv_store_unsupported(k, v)):
+        C.kv_cache_store(k, v, k_cache.data, v_cache.data, k_cache.scale, v_cache.scale, start, rows)
+        return
+    _kv_store_ref(k, v, k_cache, v_cache, start, rows)
+
+
+def kv_cache_load(cache: Fp8KV, end: int) -> Tensor:
+    """Rows [0, end) of an fp8 [B, S, Hkv, D] cache dequantised to bf16 [B, end, Hkv, D]: bf16(float(q) * s).  The
+    scratch the prefill's attention reads."""
+    D = cache.data.shape[-1]
+    if C := _kernels("kv_cache_load", cache.data, dtypes=_KV_DTYPES,
+                     unsupported=None if D % 8 == 0 else "head dim not a multiple of 8"):
+        return C.kv_cache_load(cache.data, cache.scale, end)
+    return cache.values(end).to(torch.bfloat16)
+
+
+def _kv_pair(k_cache, v_cache):
+    """(k data, v data, dtypes the kernels admit, scale kwargs) of a bf16 or Fp8KV cache pair."""
+    if isinstance(k_cache, Fp8KV):
+        return k_cache.data, v_cache.data, _KV_DTYPES, {"k_scale": k_cache.scale, "v_scale": v_cache.scale}
+    return k_cache, v_cache, (torch.bfloat16,), {}
+
+
+def _decode_fp8_unsupported(D: int, k_cache) -> Optional[str]:
+    """Why the fp8 decode kernel cannot take head dim D (8-byte row pieces of 8 channels, up to 128), or None."""
+    if not isinstance(k_cache, Fp8KV) or (D % 8 == 0 and D <= 128):
+        return None
+    return "head dim not a multiple of 8 up to 128"
+
+
+# =================================================================================================
 # decode attention over a KV cache whose valid length lives on the device (serving; not differentiable)
 # =================================================================================================
 def decode_attention(q: Tensor, k_new: Tensor, v_new: Tensor, k_cache: Tensor, v_cache: Tensor, kv_len: Tensor,
@@ -880,13 +1017,19 @@ def decode_attention(q: Tensor, k_new: Tensor, v_new: Tensor, k_cache: Tensor, v
     QKV projection are fine); k/v_cache: [B, S_max, h, D], updated in place at row kv_len-1; kv_len: int32 scalar tensor
     = valid rows including the new one; because it is read on the device, one captured CUDA graph serves every decode
     position.  Returns o [B, 1, h, D].  One cache-streaming kernel: no separate cache copies, no padded tensor-core
-    attention."""
-    if C := _kernels("decode_attention", q, k_cache, v_cache):
+    attention.  With Fp8KV caches the new rows are quantised as they are appended and every query attends to the
+    cache's values float(q) * s, its own token's included."""
+    kd, vd, dtypes, scales = _kv_pair(k_cache, v_cache)
+    if C := _kernels("decode_attention", q, kd, vd, dtypes=dtypes,
+                     unsupported=lambda: _decode_fp8_unsupported(q.shape[-1], k_cache)):
         if k_new.stride() != v_new.stride() or k_new.stride(-1) != 1:      # e.g. k went through rotary, v did not
             k_new, v_new = k_new.contiguous(), v_new.contiguous()
-        return C.decode_attention(q if q.stride(-1) == 1 else q.contiguous(), k_new, v_new, k_cache, v_cache, kv_len,
-                                  scale)
+        return C.decode_attention(q if q.stride(-1) == 1 else q.contiguous(), k_new, v_new, kd, vd, kv_len,
+                                  scale, **scales)
     n = int(kv_len)
+    if scales:
+        _kv_store_ref(k_new, v_new, k_cache, v_cache, n - 1, None)
+        return _attn_ref(q, k_cache.values(n), v_cache.values(n), scale, True)[0]
     k_cache[:, n - 1:n] = k_new
     v_cache[:, n - 1:n] = v_new
     return _attn_ref(q, k_cache[:, :n], v_cache[:, :n], scale, True)[0]
@@ -909,18 +1052,23 @@ def decode_attention_gqa(qkv_new: Tensor, k_cache: Tensor, v_cache: Tensor, kv_l
     bit; None = no rotary.  The (rotated) k and v are appended to k/v_cache [B, S_max, Hkv, D] at row kv_len - 1
     (kv_len: int32 device scalar, valid rows including the new one), then query head kv * G + g attends to rows
     [0, kv_len) of K/V head kv.  One kernel launch that reads every cache row once for its whole group; one captured
-    CUDA graph serves every position.  Returns o [B, 1, Hkv * G, D]."""
+    CUDA graph serves every position.  Returns o [B, 1, Hkv * G, D].  Fp8KV caches: see `decode_attention`."""
     B, _, Hkv, P, D = qkv_new.shape
     rope = position_ids is not None
     inv_freq = _inv_freq(D, float(theta), str(qkv_new.device)) if rope else None
-    if C := _kernels("decode_attention_gqa", qkv_new, k_cache, v_cache,
+    kd, vd, dtypes, scales = _kv_pair(k_cache, v_cache)
+    if C := _kernels("decode_attention_gqa", qkv_new, kd, vd, dtypes=dtypes,
                      unsupported=lambda: _decode_gqa_unsupported(qkv_new)):
         pos = position_ids.to(torch.int64).reshape(B, 1).contiguous() if rope else None
-        return C.decode_attention_packed(qkv_new, k_cache, v_cache, kv_len, scale, pos, inv_freq)
+        return C.decode_attention_packed(qkv_new, kd, vd, kv_len, scale, pos, inv_freq, **scales)
     if rope:
         qkv_new = _rotary_ref(qkv_new, position_ids, inv_freq, False)
     q, k, v = _gqa_split(qkv_new)
     n = int(kv_len)
+    if scales:
+        _kv_store_ref(k, v, k_cache, v_cache, n - 1, None)
+        o, _ = _gqa_attn_ref(q, k_cache.values(n), v_cache.values(n), scale, True)
+        return o.reshape(B, 1, Hkv * (P - 2), D)
     k_cache[:, n - 1:n] = k
     v_cache[:, n - 1:n] = v
     o, _ = _gqa_attn_ref(q, k_cache[:, :n], v_cache[:, :n], scale, True)
@@ -977,10 +1125,15 @@ def ragged_attention(q: Tensor, k_cache: Tensor, v_cache: Tensor, seq_start: Ten
     """q: [T, h, D]; k/v_cache: [slots, h_kv, D] with h_kv dividing h (grouped-query attention: query head i reads
     cache head i // (h / h_kv)); token t attends to cache rows seq_start[t] .. seq_start[t]+ctx_len[t]-1
     (ctx_len 0 = padding token -> zeros).  `max_ctx` bounds ctx_len (sizes the score buffer).  `alibi`: optional fp32
-    [h] slopes, bias = slope * key position.  (reference: the external fused_mmha of opt_model_1d.py:151-178)"""
-    if C := _kernels("ragged_attention", q, k_cache, v_cache):
-        return C.ragged_attention(q if q.stride(-1) == 1 else q.contiguous(), k_cache, v_cache, seq_start, ctx_len,
-                                  scale, max_ctx, alibi)
+    [h] slopes, bias = slope * key position.  Fp8KV caches ([slots, h_kv, D] data): tokens attend to the values
+    float(q) * s.  (reference: the external fused_mmha of opt_model_1d.py:151-178)"""
+    kd, vd, dtypes, scales = _kv_pair(k_cache, v_cache)
+    if C := _kernels("ragged_attention", q, kd, vd, dtypes=dtypes,
+                     unsupported=lambda: None if not scales or q.shape[-1] % 8 == 0 else "head dim not a multiple of 8"):
+        return C.ragged_attention(q if q.stride(-1) == 1 else q.contiguous(), kd, vd, seq_start, ctx_len,
+                                  scale, max_ctx, alibi, **scales)
+    if scales:
+        k_cache, v_cache = k_cache.values(), v_cache.values()
     T, h, D = q.shape
     longest = int(ctx_len.max()) if T else 0
     if longest > max_ctx:
@@ -1693,6 +1846,9 @@ class _FastNamespace:
         self.norm_rows = norm_rows
         self.ragged_attention = ragged_attention
         self.linear_mxfp8 = linear_mxfp8
+        self.Fp8KV = Fp8KV
+        self.kv_cache_store = kv_cache_store
+        self.kv_cache_load = kv_cache_load
 
 
 fast = _FastNamespace(_fast_ns)

@@ -82,7 +82,7 @@ class Generator:
     @classmethod
     def load_model(cls, model_name: str, path: Optional[str] = None, tokenizer=None, **kwargs) -> "Generator":
         """Build the model and its generator (reference: Generator.load_model :88-131 -- tokenizer + model wrapper).
-        `kwargs` go to `get_model` (batch_size, max_seq_len, dtype, weight_dtype, device, group)."""
+        `kwargs` go to `get_model` (batch_size, max_seq_len, dtype, weight_dtype, kv_cache_dtype, device, group)."""
         g = get_model(model_name, path=path, dummy=path is None, **kwargs)
         g.tokenizer = tokenizer
         return g
@@ -376,10 +376,11 @@ class Generator:
 
 def get_model(model_name: str, path: Optional[str] = None, dummy: bool = True, batch_size: int = 1,
               max_seq_len: int = 2048, dtype=torch.bfloat16, weight_dtype: str = "bf16", device: str = "cuda",
-              group=None, params: Optional[Dict] = None) -> Generator:
+              group=None, params: Optional[Dict] = None, kv_cache_dtype: str = "bf16") -> Generator:
     """HF-compatible entry (reference: get_model, wrapper.py:501).  `dummy=True` (or no `path`) uses random-init
-    weights of the named architecture; `path` points to a directory of .npy weights in the reference's layout."""
-    cfg = get_config(model_name, dtype=dtype, weight_dtype=weight_dtype)
+    weights of the named architecture; `path` points to a directory of .npy weights in the reference's layout.
+    `kv_cache_dtype="fp8"` keeps the KV cache in e4m3 with per-token, per-head scales (OPTConfig.kv_cache_dtype)."""
+    cfg = get_config(model_name, dtype=dtype, weight_dtype=weight_dtype, kv_cache_dtype=kv_cache_dtype)
     if path is not None and not dummy:
         params = load_params_np(cfg, path)
     model = DecoderLM(cfg, device=device, group=group, params=params)

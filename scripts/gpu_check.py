@@ -2,7 +2,8 @@
 calls after 5 warm-ups).  The kernels' numerics are checked by the GPU tests under tests/.
 
 usage: python scripts/gpu_check.py [section ...]
-  sections: gemm_bench gemm_sweep misc attn attn_gqa moe fp8 gemv ragged llama llama_step (default: all)
+  sections: gemm_bench gemm_sweep misc attn attn_gqa moe fp8 gemv ragged llama llama_step llama_decode kv_fp8
+            (default: all)
 gemm_bench also checks the outputs it times; the exit code is non-zero if one is wrong.
 """
 import math
@@ -465,9 +466,47 @@ def sec_llama_decode():
             torch.cuda.empty_cache()
 
 
+def sec_kv_fp8():
+    """The grouped decode kernel over a bf16 and over an fp8 cache at the Llama-3-8B shape (Hkv = 8, G = 4, D = 128),
+    timed alternately (bf16, fp8, bf16, fp8; the median of each kernel's two medians), L2 flushed before each call.
+    Bytes are the cache bytes each kernel must read: per K / V row and head, D * 2 (bf16) or D + 4 (e4m3 + its fp32
+    scale); the share is of 3.35 TB/s (H100 SXM data sheet).  The fp8 cache holds the bf16 cache's rows quantised by
+    the store kernel; the two outputs are checked against each other."""
+    Hkv, G, D, theta = 8, 4, 128, 500000.0
+    scale = D ** -0.5
+    print("kv_fp8: B ctx | bf16 us GB/s share | fp8 us GB/s share | fp8 speed-up", flush=True)
+    for B in (1, 8, 32):
+        for ctx in (1024, 4096, 16384):
+            torch.manual_seed(0)
+            qkv = torch.randn(B, 1, Hkv, G + 2, D, device="cuda", dtype=torch.bfloat16)
+            kc = torch.randn(B, ctx, Hkv, D, device="cuda", dtype=torch.bfloat16)
+            vc = torch.randn_like(kc)
+            k8, v8 = ops.Fp8KV.zeros(kc.shape, "cuda"), ops.Fp8KV.zeros(kc.shape, "cuda")
+            ops.kv_cache_store(kc, vc, k8, v8, 0)
+            kv_len = torch.full((1,), ctx, dtype=torch.int32, device="cuda")
+            pos = torch.full((B, 1), ctx - 1, dtype=torch.long, device="cuda")
+            runs = {"bf16": lambda: ops.fast.decode_attention_gqa(qkv, kc, vc, kv_len, pos, scale, theta),
+                    "fp8": lambda: ops.fast.decode_attention_gqa(qkv, k8, v8, kv_len, pos, scale, theta)}
+            ts = {k: [] for k in runs}
+            for _ in range(2):
+                for k, fn in runs.items():
+                    ts[k].append(median_ms(fn, flush=True))
+            t = {k: float(np.median(v)) for k, v in ts.items()}
+            check(f"kv_fp8 B={B} ctx={ctx} fp8 vs bf16 cache", runs["fp8"]().float(), runs["bf16"]().float(), 2e-2,
+                  1e-1)
+            rows = 2 * B * ctx * Hkv
+            gbs = {"bf16": rows * D * 2 / t["bf16"] / 1e6, "fp8": rows * (D + 4) / t["fp8"] / 1e6}
+            print(f"kv_fp8: B={B:2d} ctx={ctx:5d} | {t['bf16'] * 1e3:8.1f} us {gbs['bf16']:7.0f} GB/s "
+                  f"{gbs['bf16'] / 3350:5.1%} | {t['fp8'] * 1e3:8.1f} us {gbs['fp8']:7.0f} GB/s {gbs['fp8'] / 3350:5.1%}"
+                  f" | {t['bf16'] / t['fp8']:4.2f}x", flush=True)
+            del kc, vc, k8, v8
+            torch.cuda.empty_cache()
+
+
 SECTIONS = {"gemm_bench": sec_gemm_bench, "gemm_sweep": sec_gemm_sweep, "misc": sec_misc, "attn": sec_attn,
             "attn_gqa": sec_attn_gqa, "moe": sec_moe, "fp8": sec_fp8, "gemv": sec_gemv, "ragged": sec_ragged,
-            "llama": sec_llama, "llama_step": sec_llama_step, "llama_decode": sec_llama_decode}
+            "llama": sec_llama, "llama_step": sec_llama_step, "llama_decode": sec_llama_decode,
+            "kv_fp8": sec_kv_fp8}
 
 
 def card():
