@@ -574,10 +574,14 @@ class DecoderLM:
         return [self._new_kv((num_slots + 1, self.kv_local, self.D)) for _ in self.layers]
 
     def forward_1d(self, input_ids: torch.Tensor, position: torch.Tensor, slot: torch.Tensor, seq_start: torch.Tensor,
-                   ctx_len: torch.Tensor, cache, max_ctx: int, logit_index: torch.Tensor) -> torch.Tensor:
+                   ctx_len: torch.Tensor, cache, max_ctx: int, logit_index: torch.Tensor,
+                   block_table: Optional[torch.Tensor] = None, block_size: Optional[int] = None) -> torch.Tensor:
         """One iteration over a flat batch of T tokens that belong to different sequences (new prompts and running
         decodes mixed).  input_ids/position/slot: int64 [T]; seq_start/ctx_len: int32 [T] (see KVCacheManager.
         prepare_inputs).  K/V of every token go to cache row `slot`; attention reads each sequence's rows in place.
+        A paged cache passes its int32 `block_table` and `block_size` (PagedKVCacheManager.prepare_inputs; seq_start
+        is then a row of the table).  An empty `logit_index` (a batch of prefill chunks that end no prompt) still
+        writes every token's K/V and returns no rows.
         Returns logits [len(logit_index), V_local] of the rows in `logit_index` (the last token of every sequence).
         (reference: OPTForLMModule.__call__ of opt_model_1d.py:378 with fused_mmha)"""
         cfg = self.cfg
@@ -592,9 +596,11 @@ class DecoderLM:
                 qkv = ops.fast.rotary_packed(qkv, position.view(1, T), cfg.rope_theta, False)[0]
                 self._cache_write(kc, vc, qkv[None, :, :, G], qkv[None, :, :, G + 1], slot)
                 q = qkv[:, :, :G].reshape(T, self.nh_local, self.D)
-                o = ops.fast.ragged_attention(q, kc, vc, seq_start, ctx_len, scale, max_ctx)
+                o = ops.fast.ragged_attention(q, kc, vc, seq_start, ctx_len, scale, max_ctx, None, block_table, block_size)
                 x = x + self._all_reduce(l["out"](o.reshape(T, self.nh_local * self.D)))
                 x = x + self._all_reduce(self._mlp_llama(l, ops.fast.norm_rows(x, l["ln2"])))
+            if logit_index.numel() == 0:
+                return x.new_empty(0, self.V_local)
             return self._head_llama(ops.fast.norm_rows(x.index_select(0, logit_index).contiguous(), self.final_ln))
         for l, (kc, vc) in zip(self.layers, cache):
             h = ops.fast.layer_norm(x, l["ln1"][0], l["ln1"][1], cfg.layer_norm_eps)[0]
@@ -604,7 +610,7 @@ class DecoderLM:
                 q, k = self._rotary(q[None], k[None], position.view(1, T))
                 q, k = q[0], k[0]
             self._cache_write(kc, vc, k[None], v[None], slot)
-            o = ops.fast.ragged_attention(q, kc, vc, seq_start, ctx_len, scale, max_ctx, alibi)
+            o = ops.fast.ragged_attention(q, kc, vc, seq_start, ctx_len, scale, max_ctx, alibi, block_table, block_size)
             a = l["out"](o.reshape(T, self.nh_local * self.D))
             if cfg.parallel_block:
                 x = x + self._all_reduce(a + l["fc2"](l["fc1"](h, cfg.activation)))
@@ -613,6 +619,8 @@ class DecoderLM:
             h = ops.fast.layer_norm(x, l["ln2"][0], l["ln2"][1], cfg.layer_norm_eps)[0]
             m = self._all_reduce(l["fc2"](l["fc1"](h, cfg.activation)))
             x = x + m
+        if logit_index.numel() == 0:
+            return x.new_empty(0, self.V_local)
         x = x.index_select(0, logit_index)
         x = ops.fast.layer_norm(x.contiguous(), self.final_ln[0], self.final_ln[1], cfg.layer_norm_eps)[0]
         return ops.fast.linear(x, self.head_w, self.head_b)

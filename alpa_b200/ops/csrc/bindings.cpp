@@ -326,10 +326,12 @@ std::vector<Tensor> attention_fwd(const Tensor& q, const Tensor& k, const Tensor
   return {o, lse};
 }
 
-// Attention of a ragged 1-D token batch against a slot-addressed KV cache (see ragged_attention_sm90.cu).
+// Attention of a ragged 1-D token batch against a slot-addressed KV cache (see ragged_attention_sm90.cu).  With a
+// block table the cache is paged: seq_start[t] is token t's row of the table, and key j is in block table[row][j / bs].
 Tensor ragged_attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& seq_start,
                         const Tensor& ctx_len, double scale, int64_t max_ctx, const OptTensor& alibi,
-                        const OptTensor& k_scale, const OptTensor& v_scale) {
+                        const OptTensor& k_scale, const OptTensor& v_scale, const OptTensor& block_table,
+                        int64_t block_size) {
   TORCH_CHECK(q.dim() == 3 && q.stride(2) == 1 && q.scalar_type() == at::kBFloat16, "ragged_attention: q must be bf16 [T, heads, D]");
   const bool fp8 = k_cache.scalar_type() == at::kFloat8_e4m3fn;
   TORCH_CHECK(k_cache.dim() == 3 && v_cache.dim() == 3 && (fp8 || k_cache.scalar_type() == at::kBFloat16) &&
@@ -376,6 +378,18 @@ Tensor ragged_attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_
   a.kv_stride_s = k_cache.stride(0);
   a.scale = (float)scale;
   a.group = (int)(q.size(1) / k_cache.size(1));
+  if (block_table.has_value() && block_table->defined()) {
+    const Tensor& bt = *block_table;
+    TORCH_CHECK(bt.scalar_type() == at::kInt && bt.dim() == 2 && bt.device() == q.device() && bt.stride(1) == 1,
+                "ragged_attention: block_table must be int32 CUDA [N, max_blocks] with unit inner stride");
+    TORCH_CHECK(block_size >= 1 && block_size <= 1024 && (block_size & (block_size - 1)) == 0,
+                "ragged_attention: block_size must be a power of two up to 1024");
+    TORCH_CHECK(bt.size(1) * block_size >= max_ctx, "ragged_attention: block_table has ", bt.size(1),
+                " blocks per row, too few for max_ctx ", max_ctx, " at block size ", block_size);
+    a.block_table = bt.data_ptr<int>();
+    a.bt_stride = bt.stride(0);
+    while ((int64_t{1} << a.block_log2) < block_size) ++a.block_log2;
+  }
   AB_CHECK_RC(ab_ragged_attention(&a, cur_stream()), "ab_ragged_attention");
   g_launches += 1;
   return o;
@@ -1287,7 +1301,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("ce_grad_", &ce_grad_);
   m.def("ragged_attention", &ragged_attention, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("seq_start"),
         py::arg("ctx_len"), py::arg("scale"), py::arg("max_ctx"), py::arg("alibi") = py::none(),
-        py::arg("k_scale") = py::none(), py::arg("v_scale") = py::none());
+        py::arg("k_scale") = py::none(), py::arg("v_scale") = py::none(), py::arg("block_table") = py::none(),
+        py::arg("block_size") = 0);
   m.def("dropout", &dropout);
   m.def("embedding_fwd", &embedding_fwd);
   m.def("embedding_bwd_", &embedding_bwd_);

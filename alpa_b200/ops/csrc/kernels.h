@@ -114,7 +114,7 @@ struct RaggedAttnArgs {
   const void* k_cache = nullptr;           // [slots, heads, D] bf16 or e4m3 (cache_fp8), heads*D contiguous in a row
   const void* v_cache = nullptr;
   __nv_bfloat16* o = nullptr;              // [T, heads, D]
-  const int* seq_start = nullptr;          // [T] first cache row of the token's sequence
+  const int* seq_start = nullptr;          // [T] first cache row of the token's sequence (paged: its block table row)
   const int* ctx_len = nullptr;            // [T] rows attended (0 = padding token)
   const float* alibi = nullptr;            // optional [heads] slopes: score += slope * key_position
   int T = 0, heads = 0, D = 0, max_ctx = 0;
@@ -126,6 +126,13 @@ struct RaggedAttnArgs {
   const float* k_scale = nullptr;
   const float* v_scale = nullptr;
   long long scale_stride_h = 0;
+  // Paged cache (block_table != nullptr): [N, bt_stride] int32 block ids, block size 1 << block_log2 (0..10) rows.  Key
+  // j of token t lives in row (bt[seq_start[t]][j >> block_log2] << block_log2) | (j & (block size - 1)); for fp8 the
+  // scales are indexed by that row too.  Entries are trusted like seq_start: the block allocator builds them, and
+  // every entry a token reads (j < ctx_len) must name a block inside the cache.
+  const int* block_table = nullptr;
+  long long bt_stride = 0;
+  int block_log2 = 0;
 };
 
 // Decode-step attention with fused KV-cache append (decode_attention_sm90.cu).  Grouped-query attention: query head

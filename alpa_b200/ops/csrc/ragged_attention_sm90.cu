@@ -4,9 +4,14 @@
 // `fused_mmha(qkv, bias, cache_k, cache_v)` on a flat token batch whose tokens belong to different sequences.
 //
 // Layout here: q/o are [T, heads, D]; the KV cache is [slots, heads / group, D] (grouped-query attention: query head h
-// reads cache head h / group; group = 1 is multi-head attention) and every sequence owns a contiguous slot
-// range (alpa_b200/csrc/serving_runtime.cpp).  Token t attends to cache rows [seq_start[t], seq_start[t]+ctx_len[t])
-// -- prompt tokens and decode tokens look the same, causality is encoded in ctx_len.  One CTA per (head, token):
+// reads cache head h / group; group = 1 is multi-head attention).  Token t attends to keys j < ctx_len[t] of its
+// sequence -- prompt tokens and decode tokens look the same, causality is encoded in ctx_len.  Key j lives in cache row
+//   contiguous  seq_start[t] + j                 (every sequence owns a slot range, KVCacheManager)
+//   paged       (bt[j >> log2 bs] << log2 bs) | (j & (bs - 1)), bt = row seq_start[t] of the block table
+//               (fixed-size blocks handed out on demand, PagedKVCacheManager; alpa_b200/csrc/serving_runtime.cpp)
+// The paged instantiation only changes where a key's row is: scores, softmax, the order of the P*V sums and the ALiBi
+// bias (by logical position j) are the contiguous kernel's, so both give the same bits on the same keys.
+// One CTA per (head, token):
 //   pass 1  thread-per-key dot products with 16-byte K loads -> scores in shared memory, block max / sum
 //   pass 2  thread-per-channel-pair accumulation of P*V with coalesced 4-byte V loads, key range split over groups
 // The op is bandwidth bound (it streams the sequence's K and V once per query token), so it stays on the CUDA cores.
@@ -36,7 +41,7 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
-template <typename Cache>
+template <typename Cache, bool Paged>
 __global__ void __launch_bounds__(kRaggedThreads) ragged_attention_kernel(RaggedAttnArgs a) {
   constexpr bool F8 = std::is_same_v<Cache, __nv_fp8_e4m3>;
   extern __shared__ __align__(16) float smem[];
@@ -55,7 +60,10 @@ __global__ void __launch_bounds__(kRaggedThreads) ragged_attention_kernel(Ragged
     for (int d = tid; d < D; d += kRaggedThreads) o[d] = __float2bfloat16(0.f);
     return;
   }
-  const long long row0 = a.seq_start[t];
+  // contiguous: rows are row0 + j.  paged: row0 = 0 and key j's row comes from the sequence's block table row
+  const long long row0 = Paged ? 0 : a.seq_start[t];
+  const int* bt = Paged ? a.block_table + (long long)a.seq_start[t] * a.bt_stride : nullptr;
+  const int lg = a.block_log2;
   const __nv_bfloat16* q = a.q + (long long)t * a.q_stride_t + (long long)head * a.q_stride_h;
   for (int d = tid; d < D; d += kRaggedThreads) qs[d] = __bfloat162float(q[d]) * a.scale;
   __syncthreads();
@@ -68,17 +76,19 @@ __global__ void __launch_bounds__(kRaggedThreads) ragged_attention_kernel(Ragged
   float lmax = -INFINITY;
   for (int j = tid; j < ctx; j += kRaggedThreads) {
     float s = 0.f;
+    long long r = j;
+    if constexpr (Paged) r = ((long long)__ldg(bt + (j >> lg)) << lg) | (j & ((1 << lg) - 1));
     if constexpr (F8) {
-      const uint2* kr = reinterpret_cast<const uint2*>(kbase + (long long)j * a.kv_stride_s);
+      const uint2* kr = reinterpret_cast<const uint2*>(kbase + r * a.kv_stride_s);
       for (int c = 0; c < D / 8; ++c) {
         float f[8];
         kv_fp8_unpack8(__ldg(kr + c), f);
 #pragma unroll
         for (int e = 0; e < 8; ++e) s = fmaf(f[e], qs[c * 8 + e], s);
       }
-      s *= __ldg(ks + j);                                       // score = s_k * dot(q, k8)
+      s *= __ldg(ks + r);                                       // score = s_k * dot(q, k8)
     } else {
-      const int4* kr = reinterpret_cast<const int4*>(kbase + (long long)j * a.kv_stride_s);
+      const int4* kr = reinterpret_cast<const int4*>(kbase + r * a.kv_stride_s);
       for (int c = 0; c < D / 8; ++c) {
         int4 pk = __ldg(kr + c);
         const __nv_bfloat162* k2 = reinterpret_cast<const __nv_bfloat162*>(&pk);
@@ -113,14 +123,26 @@ __global__ void __launch_bounds__(kRaggedThreads) ragged_attention_kernel(Ragged
   if (g < groups) {
     const Cache* vbase = static_cast<const Cache*>(a.v_cache) + row0 * a.kv_stride_s + (long long)kv_head * D + 2 * c;
     float acc0 = 0.f, acc1 = 0.f;
+    // paged: a thread steps through keys in order, so it keeps its current block's first row in a register and
+    // reads the table only when it enters the next block
+    int cur_blk = -1;
+    long long blk_row = 0;
     for (int j = g; j < ctx; j += groups) {
       float2 f;
       float p = sc[j];
+      long long r = j;
+      if constexpr (Paged) {
+        if ((j >> lg) != cur_blk) {
+          cur_blk = j >> lg;
+          blk_row = (long long)__ldg(bt + cur_blk) << lg;
+        }
+        r = blk_row | (j & ((1 << lg) - 1));
+      }
       if constexpr (F8) {
-        f = kv_fp8_unpack2(*reinterpret_cast<const uint16_t*>(vbase + (long long)j * a.kv_stride_s));
-        p *= __ldg(vs + j);                                     // acc += (p * s_v) * v8
+        f = kv_fp8_unpack2(*reinterpret_cast<const uint16_t*>(vbase + r * a.kv_stride_s));
+        p *= __ldg(vs + r);                                     // acc += (p * s_v) * v8
       } else {
-        f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(vbase + (long long)j * a.kv_stride_s));
+        f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(vbase + r * a.kv_stride_s));
       }
       acc0 = fmaf(p, f.x, acc0);
       acc1 = fmaf(p, f.y, acc1);
@@ -150,7 +172,11 @@ extern "C" int ab_ragged_attention(const ab::RaggedAttnArgs* a, cudaStream_t st)
   const size_t smem = sizeof(float) * ((size_t)a->D + 8 + (size_t)groups * a->D + (size_t)a->max_ctx);
   if (smem > 200 * 1024) return 4;
   if (a->cache_fp8 && (a->k_scale == nullptr || a->v_scale == nullptr)) return 7;
-  auto kernel = a->cache_fp8 ? ragged_attention_kernel<__nv_fp8_e4m3> : ragged_attention_kernel<__nv_bfloat16>;
+  const bool paged = a->block_table != nullptr;
+  if (paged && (a->block_log2 < 0 || a->block_log2 > 10 || a->bt_stride < ((long long)a->max_ctx + (1 << a->block_log2) - 1) >> a->block_log2))
+    return 8;
+  auto kernel = a->cache_fp8 ? (paged ? ragged_attention_kernel<__nv_fp8_e4m3, true> : ragged_attention_kernel<__nv_fp8_e4m3, false>)
+                             : (paged ? ragged_attention_kernel<__nv_bfloat16, true> : ragged_attention_kernel<__nv_bfloat16, false>);
   if (smem > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return 100 + (int)e;

@@ -1121,17 +1121,26 @@ def attention_cached_(q: Tensor, k_new: Tensor, v_new: Tensor, k_cache: Tensor, 
 # attention of a ragged 1-D token batch over a slot-addressed KV cache (iteration-level batching; not differentiable)
 # =================================================================================================
 def ragged_attention(q: Tensor, k_cache: Tensor, v_cache: Tensor, seq_start: Tensor, ctx_len: Tensor, scale: float,
-                     max_ctx: int, alibi: Optional[Tensor] = None) -> Tensor:
+                     max_ctx: int, alibi: Optional[Tensor] = None, block_table: Optional[Tensor] = None,
+                     block_size: Optional[int] = None) -> Tensor:
     """q: [T, h, D]; k/v_cache: [slots, h_kv, D] with h_kv dividing h (grouped-query attention: query head i reads
-    cache head i // (h / h_kv)); token t attends to cache rows seq_start[t] .. seq_start[t]+ctx_len[t]-1
-    (ctx_len 0 = padding token -> zeros).  `max_ctx` bounds ctx_len (sizes the score buffer).  `alibi`: optional fp32
-    [h] slopes, bias = slope * key position.  Fp8KV caches ([slots, h_kv, D] data): tokens attend to the values
+    cache head i // (h / h_kv)); token t attends to keys j < ctx_len[t] of its sequence (ctx_len 0 = padding token ->
+    zeros).  Key j is cache row seq_start[t] + j, or with a paged cache (`block_table` int32 [N, max_blocks],
+    `block_size` a power of two up to 1024) row block_table[seq_start[t], j // block_size] * block_size +
+    j % block_size: seq_start then names the token's row of the table.  Table entries are not checked by the kernel
+    (the block allocator builds them); the reference raises ValueError for an entry a token reads that lies outside
+    the cache's blocks [0, (slots - 1) // block_size) (the last row is the scratch row).  Paged and contiguous calls on
+    the same keys give the same bits.  `max_ctx` bounds ctx_len (sizes the score buffer).  `alibi`: optional fp32 [h]
+    slopes, bias = slope * key position j.  Fp8KV caches ([slots, h_kv, D] data): tokens attend to the values
     float(q) * s.  (reference: the external fused_mmha of opt_model_1d.py:151-178)"""
+    if (block_table is None) != (block_size is None):
+        raise ValueError("ragged_attention: a paged cache needs both block_table and block_size")
     kd, vd, dtypes, scales = _kv_pair(k_cache, v_cache)
     if C := _kernels("ragged_attention", q, kd, vd, dtypes=dtypes,
                      unsupported=lambda: None if not scales or q.shape[-1] % 8 == 0 else "head dim not a multiple of 8"):
+        paged = {} if block_table is None else {"block_table": block_table, "block_size": int(block_size)}
         return C.ragged_attention(q if q.stride(-1) == 1 else q.contiguous(), kd, vd, seq_start, ctx_len,
-                                  scale, max_ctx, alibi, **scales)
+                                  scale, max_ctx, alibi, **scales, **paged)
     if scales:
         k_cache, v_cache = k_cache.values(), v_cache.values()
     T, h, D = q.shape
@@ -1143,14 +1152,28 @@ def ragged_attention(q: Tensor, k_cache: Tensor, v_cache: Tensor, seq_start: Ten
     if n == 0:
         return torch.zeros_like(q)
     j = torch.arange(n, device=q.device)
-    idx = (seq_start.long()[:, None] + j[None, :]).clamp_(max=k_cache.shape[0] - 1)          # [T, n]
+    valid = j[None, :] < ctx_len.long()[:, None]                                                 # [T, n]
+    if block_table is None:
+        idx = (seq_start.long()[:, None] + j[None, :]).clamp_(max=k_cache.shape[0] - 1)          # [T, n]
+    else:
+        bs = int(block_size)
+        if bs < 1 or bs > 1024 or bs & (bs - 1) or block_table.shape[1] * bs < max_ctx:
+            raise ValueError(f"ragged_attention: block size {bs} is not a power of two up to 1024, or "
+                             f"{block_table.shape[1]} blocks per table row do not cover max_ctx {max_ctx}")
+        rows = block_table.long()[seq_start.long()]                                              # [T, max_blocks]
+        blk = rows.gather(1, (j // bs).clamp(max=rows.shape[1] - 1).expand(T, n))                # [T, n]
+        nblk = (k_cache.shape[0] - 1) // bs
+        bad = valid & ((blk < 0) | (blk >= nblk))
+        if bool(bad.any()):
+            raise ValueError(f"ragged_attention: block table entry {int(blk[bad][0])} lies outside the cache's "
+                             f"{nblk} blocks")
+        idx = torch.where(valid, blk * bs + j % bs, 0)
     G = h // k_cache.shape[1]
     k = k_cache[idx].float().repeat_interleave(G, dim=2)                                         # [T, n, h, D]
     v = v_cache[idx].float().repeat_interleave(G, dim=2)
     s = torch.einsum("thd,tnhd->thn", q.float() * scale, k)
     if alibi is not None:
         s = s + alibi.view(1, h, 1) * j.view(1, 1, n)
-    valid = j[None, :] < ctx_len.long()[:, None]                                                 # [T, n]
     s = s.masked_fill(~valid[:, None, :], float("-inf"))
     p = torch.softmax(s, dim=-1)
     p = torch.nan_to_num(p, nan=0.0)                                                             # padding rows

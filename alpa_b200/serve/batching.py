@@ -6,6 +6,10 @@ enter_prompts / next / update / get_results / get_latency, pad/unpad:716-738) an
 SequenceGenerator:34 generate / generate_by_batch).  The reference's cache bookkeeping lives in an external C++
 package; here it is `alpa_b200._planner.KVCacheManager` (alpa_b200/csrc/serving_runtime.cpp) and the attention over
 the ragged batch is `ops.ragged_attention` (sm_90a kernel).
+
+With `InputPoolConfig(kv_block_size=...)` the cache is paged (`PagedKVCacheManager`): sequences take fixed-size blocks
+as they grow instead of reserving their maximum length, a prompt longer than the token budget is prefilled in chunks,
+and when the blocks run out the most recently admitted sequences are preempted and later recomputed.
 """
 from __future__ import annotations
 
@@ -37,6 +41,11 @@ class Prompt:
         self.generated_ids: List[int] = []
         self.start_time: Optional[float] = None
         self.finish_time: Optional[float] = None
+        # paged cache: the tokens to prefill (the prompt, or prompt + generated after a preemption), how many of them
+        # are in the cache, and the admission order preemption picks victims by
+        self.fill_ids: List[int] = self.input_ids
+        self.filled = 0
+        self.admitted = 0
 
     @property
     def prompt_length(self) -> int:
@@ -51,7 +60,8 @@ class Prompt:
         return self.generated_ids[-1]
 
     def start(self):
-        self.start_time = time.time()
+        if self.start_time is None:               # a recomputed sequence keeps the start time of its first admission
+            self.start_time = time.time()
 
     def add_token(self, token_id: int):
         self.generated_ids.append(int(token_id))
@@ -80,6 +90,9 @@ class InputPoolConfig:
     # None = 8 on CPU, 128 on CUDA (one full GEMM row tile: decode is weight-bandwidth bound, so 128 rows cost what 16
     # do, and every kernel sees a shape it has been validated on)
     pad_multiple: Optional[int] = None
+    # None = contiguous cache (every sequence reserves its maximum length); a power of two up to 1024 = paged cache of
+    # cache_size / kv_block_size blocks taken on demand, with chunked prefill and recompute preemption
+    kv_block_size: Optional[int] = None
 
 
 class IterationLevelInputPool:
@@ -95,8 +108,20 @@ class IterationLevelInputPool:
         self.max_length = max_length
         self.max_new_tokens = max_new_tokens
         self.pad, self.eos = pad_token_id, eos_token_id
-        self.cache_manager = _planner.KVCacheManager(config.cache_size)
+        self.block_size = config.kv_block_size
+        if self.block_size is None:
+            self.cache_manager = _planner.KVCacheManager(config.cache_size)
+        else:
+            bs = self.block_size
+            if not (isinstance(bs, int) and 1 <= bs <= 1024 and bs & (bs - 1) == 0):
+                raise ValueError(f"kv_block_size must be a power of two up to 1024, got {bs!r}")
+            if config.cache_size % bs:
+                raise ValueError(f"cache_size {config.cache_size} is not a multiple of kv_block_size {bs}")
+            self.cache_manager = _planner.PagedKVCacheManager(config.cache_size // bs, bs)
         self.pad_slot = config.cache_size            # the scratch row of DecoderLM.init_cache_1d
+        self.num_preemptions = 0
+        self.peak_blocks_used = 0
+        self._admissions = 0
         self.todo: Deque[Prompt] = deque()
         self.wip: "OrderedDict[int, Prompt]" = OrderedDict()
         self.done: "OrderedDict[int, Prompt]" = OrderedDict()
@@ -115,14 +140,39 @@ class IterationLevelInputPool:
             n = min(n, prompt_len + self.max_new_tokens)
         return max(n, prompt_len + 1)
 
+    def accepts_prompt(self, prompt_len: int) -> bool:
+        """Can this pool ever serve a prompt of `prompt_len` tokens?  It must leave room to generate within the
+        per-sequence cap and the cache; a contiguous pool also prefills a prompt in one iteration."""
+        cfg = self.config
+        if prompt_len + 1 > min(cfg.max_cache_per_seq, cfg.cache_size):
+            return False
+        return self.block_size is not None or prompt_len <= cfg.batch_size
+
+    def has_room_for(self, prompt_len: int, max_length: int) -> bool:
+        """Would a new prompt still be admitted behind the queued ones in the next iteration?  Contiguous: its tokens
+        fit the token budget and its `max_length` reservation fits the cache.  Paged: the queue is empty (a long
+        prompt runs in chunks), or the queued prefill work plus this prompt fits the token budget and the free
+        blocks."""
+        if self.block_size is None:
+            budget = self.batch_size - len(self.wip) - sum(p.prompt_length for p in self.todo)
+            return prompt_len <= budget and self.cache_manager.can_allocate(
+                [p.max_length for p in self.todo] + [max_length])
+        if not self.todo:
+            return True
+        pending = [len(p.fill_ids) - p.filled for p in self.todo] + [prompt_len]
+        blocks = sum(self.cache_manager.blocks_needed(p.sentence_id, len(p.fill_ids) - p.filled) for p in self.todo)
+        blocks += -(-prompt_len // self.block_size) + len(self.wip)           # one block per decoder at most
+        return sum(pending) <= self.batch_size - len(self.wip) and blocks <= self.cache_manager.num_free_blocks
+
     def enter_prompts(self, input_sequences: Sequence[Sequence[int]],
                       max_lengths: Optional[Sequence[int]] = None) -> List[int]:
         """Queue prompts; `max_lengths[i]` (prompt + generated) overrides the pool-wide limits for sequence i."""
         ids = []
+        paged = self.block_size is not None
         for i, seq in enumerate(input_sequences):
             if len(seq) == 0:
                 raise ValueError("empty prompt")
-            if len(seq) > self.batch_size:
+            if len(seq) > self.batch_size and not paged:
                 raise ValueError(f"prompt of {len(seq)} tokens exceeds the per-iteration token budget {self.batch_size}")
             cap = self.config.max_cache_per_seq
             if len(seq) >= cap:
@@ -131,7 +181,13 @@ class IterationLevelInputPool:
             # the attention kernel is launched with max_ctx = max_cache_per_seq: a longer reservation would make it
             # drop the newest keys silently, so the reservation is clamped (generation stops at the cap)
             need = min(need, cap)
-            if need > self.cache_size:
+            if paged:
+                # nothing is reserved; a sequence may grow to the whole cache, never further (it could not be served)
+                if len(seq) >= self.cache_size:
+                    raise ValueError(f"prompt of {len(seq)} tokens leaves no room to generate in a cache of "
+                                     f"{self.cache_size} tokens")
+                need = min(need, self.cache_size)
+            elif need > self.cache_size:
                 raise ValueError(f"prompt needs {need} cache slots, the cache has {self.cache_size}")
             sid = self._next_id
             self._next_id += 1
@@ -143,6 +199,8 @@ class IterationLevelInputPool:
     def next(self) -> Dict:
         """Admit as many queued prompts (FIFO) as the token budget and the cache allow, then lay the batch out:
         all tokens of each new prompt, one token per running sequence, padding."""
+        if self.block_size is not None:
+            return self._next_paged()
         decoding = list(self.wip.values())
         budget = self.batch_size - len(decoding)
         admitted: List[Prompt] = []
@@ -159,14 +217,84 @@ class IterationLevelInputPool:
             self.cache_manager.allocate(p.sentence_id, p.max_length)
             p.start()
         tokens = [t for p in admitted for t in p.input_ids] + [p.last_generated_id for p in decoding]
-        mult = max(1, self.config.pad_multiple or 8)
-        width = min(self.batch_size, max(mult, (len(tokens) + mult - 1) // mult * mult)) if mult > 1 else len(tokens)
-        width = max(width, len(tokens))
+        width = self._width(len(tokens))
         idx = self.cache_manager.prepare_inputs([p.sentence_id for p in admitted], [p.prompt_length for p in admitted],
                                                 [p.sentence_id for p in decoding], width, self.pad_slot)
         tokens = tokens + [self.pad] * (width - len(tokens))
         self._current = admitted + decoding
         return {"input_ids": tokens, "num_new_prompts": len(admitted), "num_decoding": len(decoding), **idx}
+
+    def _width(self, n_tokens: int) -> int:
+        mult = max(1, self.config.pad_multiple or 8)
+        width = min(self.batch_size, max(mult, (n_tokens + mult - 1) // mult * mult)) if mult > 1 else n_tokens
+        return max(width, n_tokens)
+
+    def _preempt(self, p: Prompt):
+        """Return a running sequence's blocks and queue it at the front; it is recomputed from prompt + generated."""
+        self.cache_manager.free(p.sentence_id)
+        self.wip.pop(p.sentence_id, None)
+        if p in self.todo:
+            self.todo.remove(p)
+        p.fill_ids = p.input_ids + p.generated_ids
+        p.filled = 0
+        p.status = PromptStatus.PROMPT
+        self.todo.appendleft(p)
+        self.num_preemptions += 1
+
+    def _next_paged(self) -> Dict:
+        """Paged iteration: secure one slot per decoding sequence (preempting the most recently admitted sequences
+        while the blocks do not suffice), then admit prefill work FIFO while the token budget and the free blocks
+        allow; a prefill that does not fit runs as a chunk and continues in the next iteration."""
+        cm, bs = self.cache_manager, self.block_size
+        preempted = False
+        while True:
+            decoding = list(self.wip.values())
+            need = sum(cm.blocks_needed(p.sentence_id, 1) for p in decoding)
+            if need <= cm.num_free_blocks:
+                break
+            holders = decoding + [p for p in self.todo if cm.has(p.sentence_id)]
+            self._preempt(max(holders, key=lambda p: p.admitted))
+            preempted = True
+        free = cm.num_free_blocks - need
+        budget = self.batch_size - len(decoding)
+        chunks: List[tuple] = []                       # (prompt, tokens this iteration)
+        # no prefill in an iteration that had to preempt: the freed blocks would be taken back at once
+        for p in ([] if preempted else self.todo):
+            take = min(len(p.fill_ids) - p.filled, budget)
+            room = free * bs
+            if cm.has(p.sentence_id):                  # the unused rows of its last block
+                room += -cm.length(p.sentence_id) % bs
+            take = min(take, room)
+            if take <= 0:
+                break
+            chunks.append((p, take))
+            budget -= take
+            free -= cm.blocks_needed(p.sentence_id, take)
+            if p.filled + take < len(p.fill_ids):
+                break
+        ends = []
+        for p, take in chunks:
+            if not cm.has(p.sentence_id):
+                cm.allocate(p.sentence_id)
+                self._admissions += 1
+                p.admitted = self._admissions
+                p.start()
+            ends.append(p.filled + take == len(p.fill_ids))
+        tokens = [t for p, take in chunks for t in p.fill_ids[p.filled:p.filled + take]]
+        tokens += [p.last_generated_id for p in decoding]
+        width = self._width(len(tokens))
+        mb = -(-self.config.max_cache_per_seq // bs)   # the kernel's table covers max_ctx = max_cache_per_seq keys
+        idx = cm.prepare_inputs([p.sentence_id for p, _ in chunks], [take for _, take in chunks],
+                                [p.sentence_id for p in decoding], width, self.pad_slot, ends, mb)
+        for p, take in chunks:
+            p.filled += take
+        for p, end in zip([p for p, _ in chunks], ends):
+            if end:
+                self.todo.remove(p)
+        self.peak_blocks_used = max(self.peak_blocks_used, cm.num_blocks - cm.num_free_blocks)
+        tokens = tokens + [self.pad] * (width - len(tokens))
+        self._current = [p for (p, _), end in zip(chunks, ends) if end] + decoding
+        return {"input_ids": tokens, "num_new_prompts": sum(ends), "num_decoding": len(decoding), **idx}
 
     def _should_stop(self, p: Prompt, token: int) -> bool:
         if token == self.eos:
@@ -240,22 +368,29 @@ class SequenceGenerator:
         t = lambda x, dt: torch.tensor(x, dtype=dt, device=dev)  # noqa: E731
         return (t(batch["input_ids"], torch.long), t(batch["position"], torch.long), t(batch["slot"], torch.long),
                 t(batch["seq_start"], torch.int32), t(batch["ctx_len"], torch.int32),
-                t(batch["logit_index"], torch.long))
+                t(batch["logit_index"], torch.long),
+                t(batch["block_table"], torch.int32) if "block_table" in batch else None)
 
     def step(self, pool: IterationLevelInputPool, sampler=None) -> int:
         """Run one iteration for `pool`; returns the number of sequences that produced a token.  `sampler(logits
         [n, V]) -> ids [n]` replaces greedy argmax."""
         batch = pool.next()
         n = len(batch["logit_index"])
-        if n == 0:
+        if batch["num_tokens"] == 0:
             pool.update([])
             return 0
-        ids, pos, slot, seq_start, ctx_len, logit_index = self._to_dev(batch)
+        ids, pos, slot, seq_start, ctx_len, logit_index, block_table = self._to_dev(batch)
         m = self.model
-        logits = m.forward_1d(ids, pos, slot, seq_start, ctx_len, self.cache, pool.config.max_cache_per_seq, logit_index)
-        logits = m.gather_logits(logits)
-        nxt = logits.argmax(dim=-1) if sampler is None else sampler(logits)
-        pool.update(nxt.tolist())
+        paged = {} if block_table is None else {"block_table": block_table, "block_size": pool.block_size}
+        # a paged batch of prefill chunks that end no prompt has no logit rows, but its K/V must still be written
+        logits = m.forward_1d(ids, pos, slot, seq_start, ctx_len, self.cache, pool.config.max_cache_per_seq, logit_index,
+                              **paged)
+        if n:
+            logits = m.gather_logits(logits)
+            nxt = logits.argmax(dim=-1) if sampler is None else sampler(logits)
+            pool.update(nxt.tolist())
+        else:
+            pool.update([])
         self.iterations += 1
         self.tokens_processed += batch["num_tokens"]
         return n

@@ -105,8 +105,7 @@ class LangModelWorker:
             raise ValueError("need 0 <= top_p <= 1 and temperature >= 0")
         if len(prompt_ids) == 0:
             raise ValueError("empty prompt")
-        cfg = self.pool.config
-        if len(prompt_ids) + 1 > min(cfg.max_cache_per_seq, cfg.cache_size) or len(prompt_ids) > cfg.batch_size:
+        if not self.pool.accepts_prompt(len(prompt_ids)):
             raise ValueError("prompt too long for this worker")
         max_tokens = max(1, min(int(max_tokens), self.max_new_tokens_limit))
         self._uid += 1
@@ -245,8 +244,6 @@ class LangModelWorker:
         """Move requests from the scheduler into the pool while they fit; stop at the first logprob request (served
         by the caller) or the first generate request that has to wait (returned to the front of the queue)."""
         pool = self.pool
-        pending_tokens = sum(p.prompt_length for p in pool.todo)
-        pending_cache = [p.max_length for p in pool.todo]
         while not self.request_queue.empty():
             entry = self.request_queue.get_nowait()
             item = self._unwrap(entry)
@@ -254,15 +251,12 @@ class LangModelWorker:
                 return item
             need = max(min(len(item.prompt_ids) + item.max_tokens, pool.config.max_cache_per_seq, pool.cache_size),
                        len(item.prompt_ids) + 1)
-            budget = pool.batch_size - len(pool.wip) - pending_tokens
-            if len(item.prompt_ids) > budget or not pool.cache_manager.can_allocate(pending_cache + [need]):
+            if not pool.has_room_for(len(item.prompt_ids), need):
                 self.request_queue.put_nowait_special(lambda s, x: s.appendleft(x), entry)
                 self.request_queue.task_done()            # the re-queued entry is counted again by put_nowait_special
                 return None
             sid = pool.enter_prompts([item.prompt_ids], max_lengths=[need])[0]     # stops after item.max_tokens tokens
             self._running[sid] = item
-            pending_tokens += len(item.prompt_ids)
-            pending_cache.append(need)
         return None
 
     def _score(self, item: LogprobsItem) -> Dict:

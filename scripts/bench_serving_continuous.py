@@ -6,6 +6,16 @@ runs until its longest request finishes; the continuous engine retires requests 
 
     python scripts/bench_serving_continuous.py --model opt-125m --device cpu --requests 16      # smoke run on CPU
     python scripts/bench_serving_continuous.py --model opt-2.7b --weight-dtype fp8 --requests 256 (on an H100)
+
+Paged against contiguous KV cache under one KV budget, where every request declares a cap above its true length:
+
+    python scripts/bench_serving_continuous.py --model llama-3-8b --kv-block-size 0,16 --cache-tokens 32768 \
+        --max-tokens 512 --min-new 16 --max-new 256
+
+`--kv-block-size` alternates the modes (0 = contiguous) in one process on one model.  With `--max-tokens` each request
+declares prompt + max_tokens as its length; its true output length is still drawn from [min_new, max_new], and the
+sampler emits end-of-sequence there (the weights are random, so the model never would).  A contiguous cache reserves
+the declared length, a paged one takes blocks as tokens arrive.
 """
 import argparse
 import json
@@ -32,13 +42,21 @@ def main():
     p.add_argument("--batch-tokens", type=int, default=2048)
     p.add_argument("--static-batch", type=int, default=8)
     p.add_argument("--layers", type=int, default=None, help="override the layer count (smoke runs)")
+    p.add_argument("--kv-cache-dtype", default="bf16", choices=["bf16", "fp8"])
+    p.add_argument("--kv-block-size", default="0",
+                   help="comma list of KV block sizes, run alternately; 0 = contiguous cache")
+    p.add_argument("--cache-tokens", type=int, default=None,
+                   help="KV cache size in tokens (default: every request's full length at once)")
+    p.add_argument("--max-tokens", type=int, default=None,
+                   help="the generation cap every request declares (default: its true output length)")
     args = p.parse_args()
+    from alpa_b200 import ops
     from alpa_b200.model.opt_model import DecoderLM, get_config
     from alpa_b200.serve.batching import InputPoolConfig, IterationLevelInputPool, SequenceGenerator
     from alpa_b200.serve.generator import Generator
     dev = torch.device(args.device)
     dtype = torch.bfloat16 if dev.type == "cuda" else torch.float32
-    cfg = get_config(args.model, dtype=dtype, weight_dtype=args.weight_dtype)
+    cfg = get_config(args.model, dtype=dtype, weight_dtype=args.weight_dtype, kv_cache_dtype=args.kv_cache_dtype)
     if args.layers:
         cfg.num_hidden_layers = args.layers
     model = DecoderLM(cfg, device=dev, seed=0)
@@ -52,24 +70,54 @@ def main():
             torch.cuda.synchronize()
 
     # ---- continuous batching
-    per_seq = args.max_prompt + args.max_new + 1
-    pc = InputPoolConfig(batch_size=args.batch_tokens, cache_size=min(per_seq * args.requests, 1 << 20),
-                         max_cache_per_seq=per_seq)
-    eng = SequenceGenerator(model, pc)
+    per_seq = args.max_prompt + max(args.max_new, args.max_tokens or 0) + 1
+    cache_tokens = args.cache_tokens or min(per_seq * args.requests, 1 << 20)
+    declared = [len(r[0]) + (args.max_tokens or r[1]) for r in reqs]
+    eos = 2
+    modes = [int(b) for b in args.kv_block_size.split(",")]
+    engines = {}
+    for bs in modes:
+        pc = InputPoolConfig(batch_size=args.batch_tokens, cache_size=cache_tokens, max_cache_per_seq=per_seq,
+                             kv_block_size=bs or None)
+        engines[bs] = SequenceGenerator(model, pc)
 
-    def run_continuous():
-        pool = IterationLevelInputPool(pc, pad_token_id=cfg.pad_token_id, eos_token_id=-1)
-        pool.enter_prompts([r[0] for r in reqs], max_lengths=[len(r[0]) + r[1] for r in reqs])
+    def run_continuous(bs):
+        eng = engines[bs]
+        pool = IterationLevelInputPool(eng.pool_config, pad_token_id=cfg.pad_token_id,
+                                       eos_token_id=eos if args.max_tokens else -1)
+        ids = pool.enter_prompts([r[0] for r in reqs], max_lengths=declared)
+        true_len = {sid: r[1] for sid, r in zip(ids, reqs)}
+        stats = {"decode_iterations": 0, "decode_rows": 0}
+
+        def stop_at_true_length(logits):
+            rows = pool._current
+            # decode rows: sequences that were decoding before this iteration (not a preempted sequence's re-prefill)
+            decoding = sum(1 for p in rows if p.sentence_id in pool.wip)
+            stats["decode_iterations"] += 1 if decoding else 0
+            stats["decode_rows"] += decoding
+            logits = logits.clone()
+            logits[:, eos] = float("-inf")
+            nxt = logits.argmax(-1)
+            for r, p in enumerate(rows):
+                if p.generation_length + 1 >= true_len[p.sentence_id]:
+                    nxt[r] = eos
+            return nxt
         sync()
         t0 = time.perf_counter()
         while not pool.is_finished():
-            eng.step(pool)
+            eng.step(pool, stop_at_true_length if args.max_tokens else None)
         sync()
-        return time.perf_counter() - t0, pool.get_latency()
-    run_continuous()                                    # warm-up
-    it0 = eng.iterations
-    t_cont, lat_cont = run_continuous()
-    iters = eng.iterations - it0
+        return time.perf_counter() - t0, pool.get_latency(), pool, stats
+
+    results = {bs: [] for bs in modes}
+    for bs in modes:                                    # warm-up
+        run_continuous(bs)
+    for _ in range(2 if len(modes) > 1 else 1):         # alternate the modes
+        for bs in modes:
+            it0 = engines[bs].iterations
+            t, lat, pool, st = run_continuous(bs)
+            results[bs].append((t, lat, engines[bs].iterations - it0, pool, st))
+    t_cont, lat_cont, iters, _, _ = min(results[modes[0]], key=lambda r: r[0])
 
     # ---- static padded batches (sorted by prompt length to be generous to the baseline)
     gen = Generator(model, args.static_batch, per_seq + 8)
@@ -100,6 +148,15 @@ def main():
         "static_padded": {"tokens_per_s": total_new / t_stat, "seconds": t_stat, "batch": args.static_batch,
                           "mean_latency_s": sum(lat_stat) / len(lat_stat), "p90_latency_s": pct(lat_stat, 0.9)},
         "speedup": t_stat / t_cont, "requests": args.requests, "generated_tokens": total_new,
+        "kv_cache": [{"kv_block_size": bs or None, "tokens_per_s": total_new / t, "seconds": t, "iterations": it,
+                      "mean_latency_s": sum(lat) / len(lat), "p90_latency_s": pct(lat, 0.9),
+                      "mean_seqs_per_decode_iteration": st["decode_rows"] / max(1, st["decode_iterations"])
+                      if args.max_tokens else None,
+                      "preemptions": pool.num_preemptions, "peak_blocks": pool.peak_blocks_used if bs else None,
+                      "cache_tokens": cache_tokens, "cache_bytes": ops.kv_cache_nbytes(engines[bs].cache),
+                      "kv_cache_dtype": args.kv_cache_dtype}
+                     for bs in modes for t, lat, it, pool, st in [min(results[bs], key=lambda r: r[0])]],
+        "declared_max_tokens": args.max_tokens,
         "prompt_len_range": [args.min_prompt, args.max_prompt], "new_tokens_range": [args.min_new, args.max_new],
         "weight_dtype": args.weight_dtype, "device": str(dev), "data": "synthetic prompts, random-init weights"}))
 

@@ -3,6 +3,7 @@ calls after 5 warm-ups).  The kernels' numerics are checked by the GPU tests und
 
 usage: python scripts/gpu_check.py [section ...]
   sections: gemm_bench gemm_sweep misc attn attn_gqa moe fp8 gemv ragged llama llama_step llama_decode kv_fp8
+            ragged_paged
             (default: all)
 gemm_bench also checks the outputs it times; the exit code is non-zero if one is wrong.
 """
@@ -503,10 +504,83 @@ def sec_kv_fp8():
             torch.cuda.empty_cache()
 
 
+def _scatter_blocks(c, perm, bs):
+    """A copy of slot-addressed cache c whose block perm[L] holds c's block L (the scratch row stays last)."""
+    nblk = perm.numel()
+    if isinstance(c, torch.Tensor):
+        out = torch.empty_like(c)
+        out[:nblk * bs].view(nblk, -1)[perm.long()] = c[:nblk * bs].view(nblk, -1)
+        return out
+    data = torch.empty_like(c.data.view(torch.uint8))
+    data[:nblk * bs].view(nblk, -1)[perm.long()] = c.data.view(torch.uint8)[:nblk * bs].view(nblk, -1)
+    scale = torch.empty_like(c.scale)
+    H = scale.shape[0]
+    scale[:, :nblk * bs].view(H, nblk, bs)[:, perm.long()] = c.scale[:, :nblk * bs].view(H, nblk, bs)
+    return ops.Fp8KV(data.view(torch.float8_e4m3fn), scale)
+
+
+def sec_ragged_paged():
+    """The ragged kernel over a paged cache against the contiguous kernel on the same logical keys, at the Llama-3-8B
+    attention shape (h = 32, Hkv = 8, D = 128): 64 and 256 decode tokens, each with its own sequence of 1024 / 4096 /
+    16384 keys, and one 512-token prompt chunk at keys 3585..4096.  The contiguous cache gives sequence i rows
+    [i * ctx, (i + 1) * ctx); the paged cache holds the same keys in blocks scattered by a random permutation, read
+    through the matching table.  Timed alternately (contiguous, paged, twice; the median of each kernel's two
+    medians), L2 flushed before each call.  Bytes are the K and V bytes of each token's keys, counted once per token
+    (the 4 query heads of a group share them): per row and head D * 2 (bf16) or D + 4 (e4m3 and its fp32 scale).  The
+    two outputs must be bitwise equal."""
+    h, Hkv, D = 32, 8, 128
+    scale = D ** -0.5
+    print("ragged_paged: cache T ctx bs | contiguous us GB/s | paged us GB/s | paged / contiguous time", flush=True)
+    cases = [(T, ctx, False) for T in (64, 256) for ctx in (1024, 4096, 16384)] + [(512, 4096, True)]
+    for cache in ("bf16", "fp8"):
+        for T, ctx, chunk in cases:
+            torch.manual_seed(0)
+            nseq = 1 if chunk else T
+            slots = nseq * ctx
+            q = torch.randn(T, h, D, device="cuda", dtype=torch.bfloat16)
+            if cache == "bf16":
+                kc = torch.randn(slots + 1, Hkv, D, device="cuda", dtype=torch.bfloat16)
+                vc = torch.randn_like(kc)
+            else:
+                kc, vc = ops.Fp8KV.zeros((slots + 1, Hkv, D), "cuda"), ops.Fp8KV.zeros((slots + 1, Hkv, D), "cuda")
+                for r0 in range(0, slots, 1 << 19):
+                    n = min(1 << 19, slots - r0)
+                    k = torch.randn(1, n, Hkv, D, device="cuda", dtype=torch.bfloat16)
+                    ops.kv_cache_store(k, torch.randn_like(k), kc, vc, 0, torch.arange(r0, r0 + n, device="cuda"))
+            if chunk:
+                cl = torch.arange(ctx - T + 1, ctx + 1, dtype=torch.int32, device="cuda")
+                seq = torch.zeros(T, dtype=torch.int32, device="cuda")
+            else:
+                cl = torch.full((T,), ctx, dtype=torch.int32, device="cuda")
+                seq = torch.arange(T, dtype=torch.int32, device="cuda")
+            row_bytes = Hkv * (D * 2 if cache == "bf16" else D + 4)
+            nbytes = 2 * row_bytes * int(cl.sum())
+            for bs in (16, 64):
+                perm = torch.randperm(slots // bs, device="cuda").to(torch.int32)
+                kp, vp = _scatter_blocks(kc, perm, bs), _scatter_blocks(vc, perm, bs)
+                table = perm.view(nseq, ctx // bs)
+                runs = {"contiguous": lambda: ops.fast.ragged_attention(q, kc, vc, seq * ctx, cl, scale, ctx),
+                        "paged": lambda: ops.fast.ragged_attention(q, kp, vp, seq, cl, scale, ctx, None, table, bs)}
+                check(f"ragged_paged {cache} T={T} ctx={ctx} bs={bs} paged == contiguous bitwise",
+                      runs["paged"](), runs["contiguous"](), 0, 0)
+                ts = {k: [] for k in runs}
+                for _ in range(2):
+                    for k, fn in runs.items():
+                        ts[k].append(median_ms(fn, flush=True))
+                t = {k: float(np.median(v)) for k, v in ts.items()}
+                cols = " | ".join(f"{t[k] * 1e3:8.1f} us {nbytes / t[k] / 1e6:6.0f} GB/s" for k in runs)
+                print(f"ragged_paged: {cache:4s} T={T:3d} ctx={ctx:5d}{' chunk' if chunk else '      '} bs={bs:2d} | "
+                      f"{cols} | {t['paged'] / t['contiguous']:.3f}", flush=True)
+                del kp, vp, runs
+                torch.cuda.empty_cache()
+            del kc, vc
+            torch.cuda.empty_cache()
+
+
 SECTIONS = {"gemm_bench": sec_gemm_bench, "gemm_sweep": sec_gemm_sweep, "misc": sec_misc, "attn": sec_attn,
             "attn_gqa": sec_attn_gqa, "moe": sec_moe, "fp8": sec_fp8, "gemv": sec_gemv, "ragged": sec_ragged,
             "llama": sec_llama, "llama_step": sec_llama_step, "llama_decode": sec_llama_decode,
-            "kv_fp8": sec_kv_fp8}
+            "kv_fp8": sec_kv_fp8, "ragged_paged": sec_ragged_paged}
 
 
 def card():
