@@ -22,7 +22,7 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Tuple
 
 import torch
 import torch.distributed as dist
@@ -575,13 +575,19 @@ class DecoderLM:
 
     def forward_1d(self, input_ids: torch.Tensor, position: torch.Tensor, slot: torch.Tensor, seq_start: torch.Tensor,
                    ctx_len: torch.Tensor, cache, max_ctx: int, logit_index: torch.Tensor,
-                   block_table: Optional[torch.Tensor] = None, block_size: Optional[int] = None) -> torch.Tensor:
+                   block_table: Optional[torch.Tensor] = None, block_size: Optional[int] = None,
+                   chunks: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None,
+                   n_prefill: int = 0) -> torch.Tensor:
         """One iteration over a flat batch of T tokens that belong to different sequences (new prompts and running
         decodes mixed).  input_ids/position/slot: int64 [T]; seq_start/ctx_len: int32 [T] (see KVCacheManager.
         prepare_inputs).  K/V of every token go to cache row `slot`; attention reads each sequence's rows in place.
         A paged cache passes its int32 `block_table` and `block_size` (PagedKVCacheManager.prepare_inputs; seq_start
         is then a row of the table).  An empty `logit_index` (a batch of prefill chunks that end no prompt) still
         writes every token's K/V and returns no rows.
+        `chunks` = (chunk_start, chunk_len, chunk_pos) int32 [P] of the batch's P prefill entries (prefix caching,
+        PagedKVCacheManager.prepare_inputs) and `n_prefill` their total token count: those tokens, which come first,
+        attend through `ops.paged_prefill_attention`, the decode and padding tokens after them through
+        `ops.ragged_attention`.
         Returns logits [len(logit_index), V_local] of the rows in `logit_index` (the last token of every sequence).
         (reference: OPTForLMModule.__call__ of opt_model_1d.py:378 with fused_mmha)"""
         cfg = self.cfg
@@ -589,6 +595,22 @@ class DecoderLM:
         x = self._embed(input_ids.view(1, T), position.view(1, T))[0]          # [T, H]
         scale = 1.0 / math.sqrt(self.D)
         alibi = self.alibi.float().contiguous() if self.alibi is not None else None
+        if chunks is not None and alibi is not None:
+            raise ValueError("the paged prefill kernel takes no ALiBi")
+
+        def attend(q, kc, vc, q_pre=None):
+            # q [T, h, D] (q_pre: a view of its prefill rows the kernel can read in place, e.g. the grouped projection)
+            if chunks is None or n_prefill == 0:
+                return ops.fast.ragged_attention(q, kc, vc, seq_start, ctx_len, scale, max_ctx, alibi, block_table,
+                                                 block_size)
+            o = ops.fast.paged_prefill_attention(q[:n_prefill] if q_pre is None else q_pre, kc, vc, block_table,
+                                                 block_size, *chunks, scale, max_ctx)
+            if n_prefill == T:
+                return o
+            r = ops.fast.ragged_attention(q[n_prefill:], kc, vc, seq_start[n_prefill:], ctx_len[n_prefill:], scale,
+                                          max_ctx, None, block_table, block_size)
+            return torch.cat([o, r])
+
         if cfg.arch == "llama":
             G = cfg.num_attention_heads // cfg.kv_heads
             for l, (kc, vc) in zip(self.layers, cache):
@@ -596,7 +618,7 @@ class DecoderLM:
                 qkv = ops.fast.rotary_packed(qkv, position.view(1, T), cfg.rope_theta, False)[0]
                 self._cache_write(kc, vc, qkv[None, :, :, G], qkv[None, :, :, G + 1], slot)
                 q = qkv[:, :, :G].reshape(T, self.nh_local, self.D)
-                o = ops.fast.ragged_attention(q, kc, vc, seq_start, ctx_len, scale, max_ctx, None, block_table, block_size)
+                o = attend(q, kc, vc, qkv[:n_prefill, :, :G])
                 x = x + self._all_reduce(l["out"](o.reshape(T, self.nh_local * self.D)))
                 x = x + self._all_reduce(self._mlp_llama(l, ops.fast.norm_rows(x, l["ln2"])))
             if logit_index.numel() == 0:
@@ -610,7 +632,7 @@ class DecoderLM:
                 q, k = self._rotary(q[None], k[None], position.view(1, T))
                 q, k = q[0], k[0]
             self._cache_write(kc, vc, k[None], v[None], slot)
-            o = ops.fast.ragged_attention(q, kc, vc, seq_start, ctx_len, scale, max_ctx, alibi, block_table, block_size)
+            o = attend(q, kc, vc)
             a = l["out"](o.reshape(T, self.nh_local * self.D))
             if cfg.parallel_block:
                 x = x + self._all_reduce(a + l["fc2"](l["fc1"](h, cfg.activation)))

@@ -395,6 +395,71 @@ Tensor ragged_attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_
   return o;
 }
 
+// Causal prefill of query chunks against a paged bf16 cache (see paged_prefill_sm90.cu).  q: [T, heads, D] or the
+// grouped view [T, kv_heads, group, D]; chunk c's keys are read through row c of the block table.  `max_keys` bounds
+// chunk_pos + chunk_len of every chunk (the descriptors stay on the device); the table must cover it.
+Tensor paged_prefill_attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& block_table,
+                               int64_t block_size, const Tensor& chunk_start, const Tensor& chunk_len,
+                               const Tensor& chunk_pos, double scale, int64_t max_keys) {
+  TORCH_CHECK((q.dim() == 3 || q.dim() == 4) && q.stride(-1) == 1 && q.scalar_type() == at::kBFloat16,
+              "paged_prefill_attention: q must be bf16 [T, heads, D] or [T, kv_heads, group, D] with unit stride in D");
+  TORCH_CHECK(k_cache.dim() == 3 && k_cache.scalar_type() == at::kBFloat16 && v_cache.scalar_type() == at::kBFloat16 &&
+                  k_cache.stride(2) == 1 && k_cache.stride(1) == k_cache.size(2) &&
+                  k_cache.stride(0) == k_cache.size(1) * k_cache.size(2) && v_cache.strides() == k_cache.strides() &&
+                  v_cache.sizes() == k_cache.sizes(),
+              "paged_prefill_attention: caches must be dense bf16 [slots, kv_heads, D]");
+  const int64_t Hkv = k_cache.size(1), D = k_cache.size(2);
+  TORCH_CHECK(D == 64 || D == 128, "paged_prefill_attention: head dim must be 64 or 128");
+  TORCH_CHECK(q.size(-1) == D && (q.dim() == 4 ? q.size(1) == Hkv : (Hkv > 0 && q.size(1) % Hkv == 0)),
+              "paged_prefill_attention: the cache's heads must divide q's heads (grouped-query attention), head dims equal");
+  TORCH_CHECK(aligned(q.data_ptr(), 16) && aligned(k_cache.data_ptr(), 16) && aligned(v_cache.data_ptr(), 16) &&
+                  q.stride(0) % 8 == 0 && q.stride(1) % 8 == 0 && (q.dim() == 3 || q.stride(2) % 8 == 0),
+              "paged_prefill_attention: q and cache must be 16-byte aligned (TMA)");
+  const int64_t N = chunk_len.numel();
+  for (const Tensor* t : {&chunk_start, &chunk_len, &chunk_pos})
+    TORCH_CHECK(t->scalar_type() == at::kInt && t->is_contiguous() && t->dim() == 1 && t->numel() == N &&
+                    t->device() == q.device(),
+                "paged_prefill_attention: chunk_start / chunk_len / chunk_pos must be contiguous int32 CUDA [N]");
+  TORCH_CHECK(block_size >= 16 && block_size <= 1024 && (block_size & (block_size - 1)) == 0,
+              "paged_prefill_attention: block_size must be a power of two from 16 to 1024");
+  TORCH_CHECK(block_table.scalar_type() == at::kInt && block_table.dim() == 2 && block_table.device() == q.device() &&
+                  block_table.stride(1) == 1 && block_table.size(0) >= N,
+              "paged_prefill_attention: block_table must be int32 CUDA [>= N, max_blocks] with unit inner stride");
+  TORCH_CHECK(block_table.size(1) * block_size >= max_keys, "paged_prefill_attention: block_table has ",
+              block_table.size(1), " blocks per row, too few for ", max_keys, " keys at block size ", block_size);
+  TORCH_CHECK(k_cache.size(0) <= INT32_MAX && q.size(0) <= INT32_MAX, "paged_prefill_attention: too many rows");
+  c10::cuda::CUDAGuard guard(q.device());
+  const int64_t G = q.dim() == 4 ? q.size(2) : q.size(1) / Hkv;
+  Tensor o = torch::empty({q.size(0), Hkv * G, D}, q.options());
+  if (q.size(0) == 0 || N == 0) return o;
+  ab::PagedPrefillArgs a;
+  a.q = bf16_ptr(q);
+  a.k_cache = bf16_ptr(k_cache);
+  a.v_cache = bf16_ptr(v_cache);
+  a.o = reinterpret_cast<__nv_bfloat16*>(o.data_ptr());
+  a.chunk_start = chunk_start.data_ptr<int>();
+  a.chunk_len = chunk_len.data_ptr<int>();
+  a.chunk_pos = chunk_pos.data_ptr<int>();
+  a.block_table = block_table.data_ptr<int>();
+  a.bt_stride = block_table.stride(0);
+  a.q_stride_t = q.stride(0);
+  if (q.dim() == 4) {
+    a.q_stride_kv = q.stride(1);
+    a.q_stride_g = q.stride(2);
+  } else {  // head kv * G + g at (kv * G + g) * stride(1)
+    a.q_stride_kv = q.stride(1) * G;
+    a.q_stride_g = q.stride(1);
+  }
+  a.T = (int)q.size(0); a.kv_heads = (int)Hkv; a.group = (int)G; a.D = (int)D;
+  a.slots = (int)k_cache.size(0); a.num_chunks = (int)N;
+  a.block_log2 = 0;
+  while ((int64_t{1} << a.block_log2) < block_size) ++a.block_log2;
+  a.scale = (float)scale;
+  AB_CHECK_RC(ab_paged_prefill(&a, cur_stream()), "ab_paged_prefill");
+  g_launches += 1;
+  return o;
+}
+
 // Sharding-invariant dropout: y = keep(seed, stream, global index) ? x / (1 - p) : 0   (dropout_sm90.cu)
 Tensor dropout(const Tensor& x_in, double p, const Tensor& seed, int64_t stream, const std::vector<int64_t>& global_shape,
                const std::vector<int64_t>& offsets) {
@@ -1303,6 +1368,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("ctx_len"), py::arg("scale"), py::arg("max_ctx"), py::arg("alibi") = py::none(),
         py::arg("k_scale") = py::none(), py::arg("v_scale") = py::none(), py::arg("block_table") = py::none(),
         py::arg("block_size") = 0);
+  m.def("paged_prefill_attention", &paged_prefill_attention, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"),
+        py::arg("block_table"), py::arg("block_size"), py::arg("chunk_start"), py::arg("chunk_len"),
+        py::arg("chunk_pos"), py::arg("scale"), py::arg("max_keys"));
   m.def("dropout", &dropout);
   m.def("embedding_fwd", &embedding_fwd);
   m.def("embedding_bwd_", &embedding_bwd_);

@@ -135,6 +135,25 @@ struct RaggedAttnArgs {
   int block_log2 = 0;
 };
 
+// Causal prefill of query chunks against a paged bf16 cache (paged_prefill_sm90.cu).  Chunk c is queries
+// [chunk_start[c], chunk_start[c] + chunk_len[c]) of q; query i of it sits at position chunk_pos[c] + i of the sequence
+// whose block table row is c, and sees that sequence's keys j <= chunk_pos[c] + i.  Key j lives in cache row
+// (bt[c][j >> block_log2] << block_log2) | (j & (block size - 1)), block size 16..1024.
+struct PagedPrefillArgs {
+  const __nv_bfloat16* q = nullptr;     // [T, kv_heads, group, D] view: query head kv * group + g
+  const __nv_bfloat16* k_cache = nullptr;  // [slots, kv_heads, D], rows dense
+  const __nv_bfloat16* v_cache = nullptr;
+  __nv_bfloat16* o = nullptr;           // [T, kv_heads * group, D] contiguous
+  const int* chunk_start = nullptr;     // [num_chunks] each
+  const int* chunk_len = nullptr;
+  const int* chunk_pos = nullptr;
+  const int* block_table = nullptr;     // [num_chunks, bt_stride] int32, entries trusted (the block allocator builds them)
+  long long bt_stride = 0;
+  long long q_stride_t = 0, q_stride_kv = 0, q_stride_g = 0;
+  int T = 0, kv_heads = 0, group = 1, D = 0, slots = 0, num_chunks = 0, block_log2 = 4;
+  float scale = 1.f;
+};
+
 // Decode-step attention with fused KV-cache append (decode_attention_sm90.cu).  Grouped-query attention: query head
 // kv * group + g (g < group) attends with K/V head kv (HF's repeat_kv order); group == 1 is multi-head attention.
 // A CTA serves a chunk of up to 8 query heads of one K/V head (ab_decode_attention_rows: the CTA rows per sequence).
@@ -231,6 +250,7 @@ int ab_attention_bwd(const ab::AttnBwdArgs* a, cudaStream_t st);
 int ab_attention_bwd_splits(const ab::AttnArgs* a);  // parts the dK / dV kernel splits each query-head group into
 int ab_gemv_decode(const ab::GemvArgs* a, cudaStream_t st);
 int ab_ragged_attention(const ab::RaggedAttnArgs* a, cudaStream_t st);
+int ab_paged_prefill(const ab::PagedPrefillArgs* a, cudaStream_t st);
 int ab_decode_attention(const ab::DecodeAttnArgs* a, cudaStream_t st);
 int ab_decode_attention_rows(const ab::DecodeAttnArgs* a);  // CTA rows per sequence (kv_heads * group chunks)
 int ab_decode_attention_chunk(const ab::DecodeAttnArgs* a);  // query heads per CTA (partials per row and split)

@@ -23,6 +23,7 @@ __all__ = [
     "attention_gqa_packed_bwd", "embedding", "embedding_bwd",
     "cross_entropy", "cross_entropy_bwd", "fused_adamw_", "pipeline_marker",
     "bmm", "moe_dispatch", "moe_combine", "moe_combine_wgrad", "moe_top2_route", "linear_fp8", "linear_decode", "RMSNormArgs", "decode_attention", "decode_attention_gqa", "ragged_attention",
+    "paged_prefill_attention",
     "Fp8KV", "kv_cache_store", "kv_cache_load", "kv_cache_nbytes",
     "attention_cached", "attention_cached_", "quantize_mxfp8", "dequantize_mxfp8", "linear_mxfp8", "mx_pack_scale_atoms",
     "mx_unpack_scale_atoms", "pack_tiles", "unpack_tiles", "packed_nbytes",
@@ -1180,6 +1181,67 @@ def ragged_attention(q: Tensor, k_cache: Tensor, v_cache: Tensor, seq_start: Ten
     return torch.einsum("thn,tnhd->thd", p, v).to(q.dtype)
 
 
+def _paged_prefill_unsupported(q: Tensor, block_size: int) -> Optional[str]:
+    """Why the paged prefill kernel cannot take these operands, or None."""
+    if q.shape[-1] not in (64, 128):
+        return "head dim not 64 or 128"
+    if block_size < 16:
+        return "block size under 16"
+    if q.stride(-1) != 1 or any(s % 8 for s in q.stride()[:-1]) or q.data_ptr() % 16:
+        return "q view not 16-byte aligned"
+    return None
+
+
+def paged_prefill_attention(q: Tensor, k_cache: Tensor, v_cache: Tensor, block_table: Tensor, block_size: int,
+                            chunk_start: Tensor, chunk_len: Tensor, chunk_pos: Tensor, scale: float,
+                            max_keys: Optional[int] = None) -> Tensor:
+    """Causal prefill of query chunks against a paged bf16 cache (prefix caching).  q: [T, h, D], or the grouped view
+    [T, h_kv, group, D] (query head kv * group + g); k/v_cache: [slots, h_kv, D] bf16; block_table: int32
+    [>= N, max_blocks]; chunk_start / chunk_len / chunk_pos: int32 [N].  Chunk c is queries [chunk_start[c],
+    chunk_start[c] + chunk_len[c]); query i of it sits at position chunk_pos[c] + i of the sequence whose table row is
+    c and attends to that sequence's keys j <= chunk_pos[c] + i, key j at row block_table[c, j // block_size] *
+    block_size + j % block_size.  Returns o [T, h, D]; rows of q outside every chunk are left undefined.
+    `max_keys` bounds chunk_pos + chunk_len (the table must cover it); None reads it from the descriptors.  Table
+    entries are trusted by the kernel; the reference raises ValueError for one outside the cache's blocks."""
+    if isinstance(k_cache, Fp8KV) or isinstance(v_cache, Fp8KV):
+        raise TypeError("paged_prefill_attention: fp8 caches are not supported")
+    if max_keys is None:
+        max_keys = int((chunk_pos.long() + chunk_len.long()).max()) if chunk_len.numel() else 0
+    bs = int(block_size)
+    if C := _kernels("paged_prefill_attention", q, k_cache, v_cache,
+                     unsupported=lambda: _paged_prefill_unsupported(q, bs)):
+        return C.paged_prefill_attention(q, k_cache, v_cache, block_table, bs, chunk_start, chunk_len, chunk_pos,
+                                         scale, int(max_keys))
+    if bs < 1 or bs > 1024 or bs & (bs - 1):
+        raise ValueError(f"paged_prefill_attention: block size {bs} is not a power of two up to 1024")
+    T, D = q.shape[0], q.shape[-1]
+    qf = q.reshape(T, -1, D).float()
+    h, h_kv = qf.shape[1], k_cache.shape[1]
+    G = h // h_kv
+    nblk = (k_cache.shape[0] - 1) // bs
+    o = torch.zeros(T, h, D, dtype=q.dtype, device=q.device)
+    for c, (s0, n, p0) in enumerate(zip(chunk_start.tolist(), chunk_len.tolist(), chunk_pos.tolist())):
+        if n == 0:
+            continue
+        keys = p0 + n
+        if keys > max_keys or keys > block_table.shape[1] * bs:
+            raise ValueError(f"paged_prefill_attention: chunk {c} reads {keys} keys, more than max_keys {max_keys} "
+                             f"or the {block_table.shape[1]} blocks of a table row")
+        j = torch.arange(keys, device=q.device)
+        blk = block_table[c].long()[j // bs]
+        if bool(((blk < 0) | (blk >= nblk)).any()):
+            raise ValueError(f"paged_prefill_attention: chunk {c} reads a block outside the cache's {nblk} blocks")
+        rows = blk * bs + j % bs
+        k = k_cache[rows].float().repeat_interleave(G, dim=1)                                    # [keys, h, D]
+        v = v_cache[rows].float().repeat_interleave(G, dim=1)
+        s = torch.einsum("ihd,jhd->hij", qf[s0:s0 + n] * scale, k)
+        qpos = p0 + torch.arange(n, device=q.device)
+        s = s.masked_fill(j[None, None, :] > qpos[None, :, None], float("-inf"))
+        p = torch.softmax(s, dim=-1)
+        o[s0:s0 + n] = torch.einsum("hij,jhd->ihd", p, v).to(q.dtype)
+    return o
+
+
 # =================================================================================================
 # sharding-invariant dropout (counter-based Philox4x32-10 keyed by seed / stream / GLOBAL element index)
 # =================================================================================================
@@ -1868,6 +1930,7 @@ class _FastNamespace:
         self.decode_attention_gqa = decode_attention_gqa
         self.norm_rows = norm_rows
         self.ragged_attention = ragged_attention
+        self.paged_prefill_attention = paged_prefill_attention
         self.linear_mxfp8 = linear_mxfp8
         self.Fp8KV = Fp8KV
         self.kv_cache_store = kv_cache_store

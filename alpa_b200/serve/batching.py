@@ -9,7 +9,10 @@ the ragged batch is `ops.ragged_attention` (sm_90a kernel).
 
 With `InputPoolConfig(kv_block_size=...)` the cache is paged (`PagedKVCacheManager`): sequences take fixed-size blocks
 as they grow instead of reserving their maximum length, a prompt longer than the token budget is prefilled in chunks,
-and when the blocks run out the most recently admitted sequences are preempted and later recomputed.
+and when the blocks run out the most recently admitted sequences are preempted and later recomputed.  With
+`prefix_caching=True` as well, full blocks are shared between sequences whose token prefixes are equal: a new or
+re-admitted prompt starts from the longest cached chain of blocks matching it and prefills only the rest, and that
+suffix attends to the cached keys through `ops.paged_prefill_attention` (sm_90a kernel).
 """
 from __future__ import annotations
 
@@ -93,6 +96,9 @@ class InputPoolConfig:
     # None = contiguous cache (every sequence reserves its maximum length); a power of two up to 1024 = paged cache of
     # cache_size / kv_block_size blocks taken on demand, with chunked prefill and recompute preemption
     kv_block_size: Optional[int] = None
+    # share full blocks between sequences with equal token prefixes (needs kv_block_size >= 16, a bf16 cache and a
+    # model without ALiBi); a prompt whose leading blocks are cached prefills only the rest
+    prefix_caching: bool = False
 
 
 class IterationLevelInputPool:
@@ -117,10 +123,17 @@ class IterationLevelInputPool:
                 raise ValueError(f"kv_block_size must be a power of two up to 1024, got {bs!r}")
             if config.cache_size % bs:
                 raise ValueError(f"cache_size {config.cache_size} is not a multiple of kv_block_size {bs}")
-            self.cache_manager = _planner.PagedKVCacheManager(config.cache_size // bs, bs)
+            if config.prefix_caching and bs < 16:
+                raise ValueError(f"prefix_caching needs kv_block_size >= 16, got {bs}")
+            self.cache_manager = _planner.PagedKVCacheManager(config.cache_size // bs, bs, config.prefix_caching)
+        if config.prefix_caching and self.block_size is None:
+            raise ValueError("prefix_caching needs a paged cache (kv_block_size)")
+        self.prefix_caching = config.prefix_caching
         self.pad_slot = config.cache_size            # the scratch row of DecoderLM.init_cache_1d
         self.num_preemptions = 0
         self.peak_blocks_used = 0
+        self.prefix_hit_tokens = 0                   # prompt tokens found in the cache, not computed
+        self.prefill_tokens_computed = 0             # prompt (and recomputed) tokens run through the model
         self._admissions = 0
         self.todo: Deque[Prompt] = deque()
         self.wip: "OrderedDict[int, Prompt]" = OrderedDict()
@@ -260,6 +273,18 @@ class IterationLevelInputPool:
         chunks: List[tuple] = []                       # (prompt, tokens this iteration)
         # no prefill in an iteration that had to preempt: the freed blocks would be taken back at once
         for p in ([] if preempted else self.todo):
+            if self.prefix_caching and budget > 0 and not cm.has(p.sentence_id):
+                # admission (or re-admission after a preemption): start from the cached blocks of its prefix; cached
+                # blocks it takes a reference on were counted as free
+                before = cm.num_free_blocks
+                hit = cm.match_prefix(p.sentence_id, p.fill_ids)
+                free -= before - cm.num_free_blocks
+                if free < 0:                           # the decoding sequences need those blocks: retry later
+                    cm.free(p.sentence_id)
+                    break
+                p.filled = hit
+                self.prefix_hit_tokens += hit
+                self._admit(p)
             take = min(len(p.fill_ids) - p.filled, budget)
             room = free * bs
             if cm.has(p.sentence_id):                  # the unused rows of its last block
@@ -276,18 +301,19 @@ class IterationLevelInputPool:
         for p, take in chunks:
             if not cm.has(p.sentence_id):
                 cm.allocate(p.sentence_id)
-                self._admissions += 1
-                p.admitted = self._admissions
-                p.start()
+                self._admit(p)
             ends.append(p.filled + take == len(p.fill_ids))
         tokens = [t for p, take in chunks for t in p.fill_ids[p.filled:p.filled + take]]
         tokens += [p.last_generated_id for p in decoding]
         width = self._width(len(tokens))
         mb = -(-self.config.max_cache_per_seq // bs)   # the kernel's table covers max_ctx = max_cache_per_seq keys
+        # with prefix caching the manager learns every written position's token, so it can index the blocks filled
+        ids = {"input_ids": tokens} if self.prefix_caching else {}
         idx = cm.prepare_inputs([p.sentence_id for p, _ in chunks], [take for _, take in chunks],
-                                [p.sentence_id for p in decoding], width, self.pad_slot, ends, mb)
+                                [p.sentence_id for p in decoding], width, self.pad_slot, ends, mb, **ids)
         for p, take in chunks:
             p.filled += take
+            self.prefill_tokens_computed += take
         for p, end in zip([p for p, _ in chunks], ends):
             if end:
                 self.todo.remove(p)
@@ -295,6 +321,11 @@ class IterationLevelInputPool:
         tokens = tokens + [self.pad] * (width - len(tokens))
         self._current = [p for (p, _), end in zip(chunks, ends) if end] + decoding
         return {"input_ids": tokens, "num_new_prompts": sum(ends), "num_decoding": len(decoding), **idx}
+
+    def _admit(self, p: Prompt):
+        self._admissions += 1
+        p.admitted = self._admissions
+        p.start()
 
     def _should_stop(self, p: Prompt, token: int) -> bool:
         if token == self.eos:
@@ -351,12 +382,26 @@ def pad(inputs, pad: int = 1) -> List[List[int]]:  # noqa: A001  (same name as t
     return [list(s) + [pad] * (n - len(s)) for s in inputs]
 
 
+def check_prefix_caching(config: InputPoolConfig, model: DecoderLM):
+    """Raise ValueError for a prefix-caching pool the model cannot serve: the suffix prefill runs on the paged
+    prefill kernel, which takes a bf16 cache without ALiBi."""
+    if not config.prefix_caching:
+        return
+    if config.kv_block_size is None or config.kv_block_size < 16:
+        raise ValueError(f"prefix_caching needs kv_block_size >= 16, got {config.kv_block_size}")
+    if model.alibi is not None:
+        raise ValueError("prefix_caching is not supported with ALiBi models (BLOOM)")
+    if model.cfg.kv_cache_dtype != "bf16":
+        raise ValueError(f"prefix_caching is not supported with a {model.cfg.kv_cache_dtype} KV cache")
+
+
 class SequenceGenerator:
     """Greedy generation with iteration-level batching over a DecoderLM (reference: wrapper_1d.SequenceGenerator:34)."""
 
     def __init__(self, model: DecoderLM, pool_config: Optional[InputPoolConfig] = None):
         self.model = model
         self.pool_config = pool_config or InputPoolConfig()
+        check_prefix_caching(self.pool_config, model)
         if self.pool_config.pad_multiple is None:
             self.pool_config.pad_multiple = 128 if model.device.type == "cuda" else 8
         self.cache = model.init_cache_1d(self.pool_config.cache_size)
@@ -382,6 +427,11 @@ class SequenceGenerator:
         ids, pos, slot, seq_start, ctx_len, logit_index, block_table = self._to_dev(batch)
         m = self.model
         paged = {} if block_table is None else {"block_table": block_table, "block_size": pool.block_size}
+        if "chunk_len" in batch and batch["chunk_len"]:
+            dev = m.device
+            paged["chunks"] = tuple(torch.tensor(batch[k], dtype=torch.int32, device=dev)
+                                    for k in ("chunk_start", "chunk_len", "chunk_pos"))
+            paged["n_prefill"] = sum(batch["chunk_len"])
         # a paged batch of prefill chunks that end no prompt has no logit rows, but its K/V must still be written
         logits = m.forward_1d(ids, pos, slot, seq_start, ctx_len, self.cache, pool.config.max_cache_per_seq, logit_index,
                               **paged)

@@ -16,6 +16,15 @@ Paged against contiguous KV cache under one KV budget, where every request decla
 declares prompt + max_tokens as its length; its true output length is still drawn from [min_new, max_new], and the
 sampler emits end-of-sequence there (the weights are random, so the model never would).  A contiguous cache reserves
 the declared length, a paged one takes blocks as tokens arrive.
+
+Prefix caching off against on, every request starting with the same 1024-token preamble:
+
+    python scripts/bench_serving_continuous.py --model llama-3-8b --kv-block-size 16 --prefix-caching \
+        --shared-prefix-tokens 1024 --requests 64 --min-prompt 16 --max-prompt 512
+
+`--prefix-caching` runs every paged block size with caching off and on, alternated in one process; each run reports
+its time to first token (p50 / p99, from the moment all requests are queued), the prompt tokens found in the cache
+and the prompt tokens computed.
 """
 import argparse
 import json
@@ -49,6 +58,10 @@ def main():
                    help="KV cache size in tokens (default: every request's full length at once)")
     p.add_argument("--max-tokens", type=int, default=None,
                    help="the generation cap every request declares (default: its true output length)")
+    p.add_argument("--prefix-caching", action="store_true",
+                   help="run every paged block size with prefix caching off and on")
+    p.add_argument("--shared-prefix-tokens", type=int, default=0,
+                   help="every prompt starts with the same preamble of this many tokens")
     args = p.parse_args()
     from alpa_b200 import ops
     from alpa_b200.model.opt_model import DecoderLM, get_config
@@ -61,7 +74,9 @@ def main():
         cfg.num_hidden_layers = args.layers
     model = DecoderLM(cfg, device=dev, seed=0)
     rnd = random.Random(0)
-    reqs = [([rnd.randint(4, cfg.vocab_size - 1) for _ in range(rnd.randint(args.min_prompt, args.max_prompt))],
+    preamble = [rnd.randint(4, cfg.vocab_size - 1) for _ in range(args.shared_prefix_tokens)]
+    reqs = [(preamble + [rnd.randint(4, cfg.vocab_size - 1)
+                         for _ in range(rnd.randint(args.min_prompt, args.max_prompt))],
              rnd.randint(args.min_new, args.max_new)) for _ in range(args.requests)]
     total_new = sum(n for _, n in reqs)
 
@@ -70,24 +85,26 @@ def main():
             torch.cuda.synchronize()
 
     # ---- continuous batching
-    per_seq = args.max_prompt + max(args.max_new, args.max_tokens or 0) + 1
+    per_seq = args.shared_prefix_tokens + args.max_prompt + max(args.max_new, args.max_tokens or 0) + 1
     cache_tokens = args.cache_tokens or min(per_seq * args.requests, 1 << 20)
     declared = [len(r[0]) + (args.max_tokens or r[1]) for r in reqs]
     eos = 2
-    modes = [int(b) for b in args.kv_block_size.split(",")]
+    # a mode is (block size, prefix caching)
+    modes = [(int(b), c) for b in args.kv_block_size.split(",")
+             for c in ((False, True) if args.prefix_caching and int(b) else (False,))]
     engines = {}
-    for bs in modes:
+    for bs, caching in modes:
         pc = InputPoolConfig(batch_size=args.batch_tokens, cache_size=cache_tokens, max_cache_per_seq=per_seq,
-                             kv_block_size=bs or None)
-        engines[bs] = SequenceGenerator(model, pc)
+                             kv_block_size=bs or None, prefix_caching=caching)
+        engines[(bs, caching)] = SequenceGenerator(model, pc)
 
-    def run_continuous(bs):
-        eng = engines[bs]
+    def run_continuous(mode):
+        eng = engines[mode]
         pool = IterationLevelInputPool(eng.pool_config, pad_token_id=cfg.pad_token_id,
                                        eos_token_id=eos if args.max_tokens else -1)
         ids = pool.enter_prompts([r[0] for r in reqs], max_lengths=declared)
         true_len = {sid: r[1] for sid, r in zip(ids, reqs)}
-        stats = {"decode_iterations": 0, "decode_rows": 0}
+        stats = {"decode_iterations": 0, "decode_rows": 0, "ttft": {}}
 
         def stop_at_true_length(logits):
             rows = pool._current
@@ -106,17 +123,23 @@ def main():
         t0 = time.perf_counter()
         while not pool.is_finished():
             eng.step(pool, stop_at_true_length if args.max_tokens else None)
+            if any(p.generation_length and p.sentence_id not in stats["ttft"]
+                   for p in list(pool.wip.values()) + list(pool.done.values())):
+                sync()
+                now = time.perf_counter() - t0
+                for p in list(pool.wip.values()) + list(pool.done.values()):
+                    stats["ttft"].setdefault(p.sentence_id, now)
         sync()
         return time.perf_counter() - t0, pool.get_latency(), pool, stats
 
-    results = {bs: [] for bs in modes}
-    for bs in modes:                                    # warm-up
-        run_continuous(bs)
+    results = {m: [] for m in modes}
+    for m in modes:                                     # warm-up
+        run_continuous(m)
     for _ in range(2 if len(modes) > 1 else 1):         # alternate the modes
-        for bs in modes:
-            it0 = engines[bs].iterations
-            t, lat, pool, st = run_continuous(bs)
-            results[bs].append((t, lat, engines[bs].iterations - it0, pool, st))
+        for m in modes:
+            it0 = engines[m].iterations
+            t, lat, pool, st = run_continuous(m)
+            results[m].append((t, lat, engines[m].iterations - it0, pool, st))
     t_cont, lat_cont, iters, _, _ = min(results[modes[0]], key=lambda r: r[0])
 
     # ---- static padded batches (sorted by prompt length to be generous to the baseline)
@@ -148,14 +171,22 @@ def main():
         "static_padded": {"tokens_per_s": total_new / t_stat, "seconds": t_stat, "batch": args.static_batch,
                           "mean_latency_s": sum(lat_stat) / len(lat_stat), "p90_latency_s": pct(lat_stat, 0.9)},
         "speedup": t_stat / t_cont, "requests": args.requests, "generated_tokens": total_new,
-        "kv_cache": [{"kv_block_size": bs or None, "tokens_per_s": total_new / t, "seconds": t, "iterations": it,
+        "kv_cache": [{"kv_block_size": bs or None, "prefix_caching": caching,
+                      "tokens_per_s": total_new / t, "seconds": t, "iterations": it,
+                      "tokens_per_s_runs": [total_new / r[0] for r in results[(bs, caching)]],
                       "mean_latency_s": sum(lat) / len(lat), "p90_latency_s": pct(lat, 0.9),
                       "mean_seqs_per_decode_iteration": st["decode_rows"] / max(1, st["decode_iterations"])
                       if args.max_tokens else None,
                       "preemptions": pool.num_preemptions, "peak_blocks": pool.peak_blocks_used if bs else None,
-                      "cache_tokens": cache_tokens, "cache_bytes": ops.kv_cache_nbytes(engines[bs].cache),
+                      "ttft_p50_s": pct(list(st["ttft"].values()), 0.5),
+                      "ttft_p99_s": pct(list(st["ttft"].values()), 0.99),
+                      "prefix_hit_tokens": pool.prefix_hit_tokens if bs else None,
+                      "prefill_tokens_computed": pool.prefill_tokens_computed if bs else None,
+                      "cache_tokens": cache_tokens, "cache_bytes": ops.kv_cache_nbytes(engines[(bs, caching)].cache),
                       "kv_cache_dtype": args.kv_cache_dtype}
-                     for bs in modes for t, lat, it, pool, st in [min(results[bs], key=lambda r: r[0])]],
+                     for bs, caching in modes
+                     for t, lat, it, pool, st in [min(results[(bs, caching)], key=lambda r: r[0])]],
+        "shared_prefix_tokens": args.shared_prefix_tokens,
         "declared_max_tokens": args.max_tokens,
         "prompt_len_range": [args.min_prompt, args.max_prompt], "new_tokens_range": [args.min_new, args.max_new],
         "weight_dtype": args.weight_dtype, "device": str(dev), "data": "synthetic prompts, random-init weights"}))

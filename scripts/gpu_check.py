@@ -3,7 +3,7 @@ calls after 5 warm-ups).  The kernels' numerics are checked by the GPU tests und
 
 usage: python scripts/gpu_check.py [section ...]
   sections: gemm_bench gemm_sweep misc attn attn_gqa moe fp8 gemv ragged llama llama_step llama_decode kv_fp8
-            ragged_paged
+            ragged_paged paged_prefill
             (default: all)
 gemm_bench also checks the outputs it times; the exit code is non-zero if one is wrong.
 """
@@ -577,10 +577,63 @@ def sec_ragged_paged():
             torch.cuda.empty_cache()
 
 
+def sec_paged_prefill():
+    """The paged prefill kernel (wgmma) against the paged ragged kernel (CUDA cores) on the same prompt chunks, at the
+    Llama-3-8B attention shape (h = 32, Hkv = 8, D = 128): one 512-token chunk at keys 3585..4096, one 2048-token chunk
+    after a 6144-token cached prefix, and a batch of four chunks of mixed lengths and prefixes; blocks of 16 and 64
+    rows scattered by a random permutation.  Timed alternately (ragged, prefill, twice; the median of each kernel's two
+    medians), L2 flushed before each call.  FLOPs are the causal ones: 4 * D * h per (query, visible key).  The share
+    of peak is against the data sheet's 989 TFLOP/s dense bf16."""
+    h, Hkv, D = 32, 8, 128
+    scale = D ** -0.5
+    print("paged_prefill: chunks bs | ragged us TFLOP/s | prefill us TFLOP/s % of 989 | ragged / prefill time",
+          flush=True)
+    cases = {"512@3584": [(3584, 512)], "2048@6144": [(6144, 2048)],
+             "mixed": [(1024, 100), (4000, 300), (0, 64), (2000, 700)]}
+    for name, chunks in cases.items():
+        torch.manual_seed(0)
+        for bs in (16, 64):
+            nb = [-(-(p + n) // bs) for p, n in chunks]
+            width = max(nb)
+            nblk = sum(nb)
+            perm = torch.randperm(nblk, device="cuda").to(torch.int32)
+            table = torch.zeros(len(chunks), width, dtype=torch.int32, device="cuda")
+            o = 0
+            for i, n in enumerate(nb):
+                table[i, :n] = perm[o:o + n]
+                o += n
+            kc = torch.randn(nblk * bs + 1, Hkv, D, device="cuda", dtype=torch.bfloat16)
+            vc = torch.randn_like(kc)
+            T = sum(n for _, n in chunks)
+            q = torch.randn(T, h, D, device="cuda", dtype=torch.bfloat16)
+            i32 = lambda x: torch.tensor(x, dtype=torch.int32, device="cuda")  # noqa: E731
+            cs = i32([sum(n for _, n in chunks[:i]) for i in range(len(chunks))])
+            cl, cp = i32([n for _, n in chunks]), i32([p for p, _ in chunks])
+            seq = i32([i for i, (_, n) in enumerate(chunks) for _ in range(n)])
+            ctx = i32([p + j + 1 for p, n in chunks for j in range(n)])
+            mc = width * bs
+            flops = 4 * D * h * int(ctx.sum())
+            runs = {"ragged": lambda: ops.fast.ragged_attention(q, kc, vc, seq, ctx, scale, mc, None, table, bs),
+                    "prefill": lambda: ops.fast.paged_prefill_attention(q, kc, vc, table, bs, cs, cl, cp, scale, mc)}
+            check(f"paged_prefill {name} bs={bs} prefill ~ ragged", runs["prefill"](), runs["ragged"](), 2e-2, 2e-2)
+            ts = {k: [] for k in runs}
+            for _ in range(2):
+                for k, fn in runs.items():
+                    ts[k].append(median_ms(fn, flush=True))
+            t = {k: float(np.median(v)) for k, v in ts.items()}
+            tf = {k: flops / t[k] / 1e9 for k in runs}
+            print(f"paged_prefill: {name:10s} bs={bs:2d} | {t['ragged'] * 1e3:9.1f} us {tf['ragged']:6.1f} | "
+                  f"{t['prefill'] * 1e3:8.1f} us {tf['prefill']:6.1f} {100 * tf['prefill'] / 989:5.1f}% | "
+                  f"{t['ragged'] / t['prefill']:.1f}x", flush=True)
+            del kc, vc, runs
+            torch.cuda.empty_cache()
+
+
 SECTIONS = {"gemm_bench": sec_gemm_bench, "gemm_sweep": sec_gemm_sweep, "misc": sec_misc, "attn": sec_attn,
             "attn_gqa": sec_attn_gqa, "moe": sec_moe, "fp8": sec_fp8, "gemv": sec_gemv, "ragged": sec_ragged,
             "llama": sec_llama, "llama_step": sec_llama_step, "llama_decode": sec_llama_decode,
-            "kv_fp8": sec_kv_fp8, "ragged_paged": sec_ragged_paged}
+            "kv_fp8": sec_kv_fp8, "ragged_paged": sec_ragged_paged,
+            "paged_prefill": sec_paged_prefill}
 
 
 def card():
