@@ -118,9 +118,8 @@ attn_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
     mma_ss_64<DP>(&sc[0][0], q_addr, kBQ * 128, sk, kAtomRows64);
     mma_sync_all();
 
-    // mask + online softmax (rows g and g + 8 of this warp; a quad of lanes shares a row)
+    // scale to exp2 and mask: key j is visible to query i iff j < Skv and, when causal, j <= i + shift
     const bool need_mask = kv0 + kTile > Skv || (a.causal && kv0 + kTile - 1 > row0 + shift);
-    float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int n = 0; n < 8; ++n) {
 #pragma unroll
@@ -131,43 +130,9 @@ attn_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
           if (key >= Skv || (a.causal && key > qrow[e >> 1] + shift)) v = -INFINITY;
         }
         sc[n][e] = v;
-        mx[e >> 1] = fmaxf(mx[e >> 1], v);
       }
     }
-    float corr[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-      const float m_new = fmaxf(m_r[r], mx[r]);
-      corr[r] = m_new == -INFINITY ? 1.f : ex2_approx(m_r[r] - m_new);
-      m_r[r] = m_new;
-      l_r[r] *= corr[r];
-    }
-    uint32_t pf[4][4];  // P as the register A operand of P V: k16 block kk = score columns [16 kk, 16 kk + 16)
-#pragma unroll
-    for (int n = 0; n < 8; ++n) {
-      float p[4];
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float m = m_r[e >> 1];
-        p[e] = m == -INFINITY ? 0.f : ex2_approx(sc[n][e] - m);
-      }
-      l_r[0] += p[0] + p[1];
-      l_r[1] += p[2] + p[3];
-      pf[n >> 1][(n & 1) * 2 + 0] = pack_bf16x2(p[0], p[1]);
-      pf[n >> 1][(n & 1) * 2 + 1] = pack_bf16x2(p[2], p[3]);
-    }
-#pragma unroll
-    for (int i = 0; i < DP / 8; ++i) {
-      o[i][0] *= corr[0];
-      o[i][1] *= corr[0];
-      o[i][2] *= corr[1];
-      o[i][3] *= corr[1];
-    }
-    wgmma_fence();
-    mma_rs<DP>(&o[0][0], pf, sv, kAtomRows64);  // O += P V
-    mma_sync_all();
+    fwd_softmax_pv<DP>(sc, o, m_r, l_r, sv);
     __syncthreads();  // every warpgroup is done with stage s: refill it with tile j + 2
     if (threadIdx.x == 0 && j + 2 < n_tiles) issue_kv(j + 2);
   }

@@ -2,8 +2,9 @@
 // uncached suffix attending to a long cached prefix).
 //
 // The structure is the forward kernel of attention_sm90.cu: one warpgroup per 64 query rows, 64-key K/V tiles in a
-// two-stage mbarrier ring, S = Q K^T with SS wgmma, O += P V with RS wgmma, online softmax in exp2 form, grouped-query
-// attention through kv_head = h / group.  What differs is where a K/V tile comes from: key j of chunk c lives in cache
+// two-stage mbarrier ring, S = Q K^T with SS wgmma, grouped-query attention through kv_head = h / group, and the same
+// online-softmax step and O += P V (fwd_softmax_pv in attention_sm90.cuh).  What differs is the mask (causal by
+// position in the sequence), the output stores, and where a K/V tile comes from: key j of chunk c lives in cache
 // row (bt[c][j >> log2 bs] << log2 bs) | (j & (bs - 1)), so a 64-key tile is one TMA box of 64 rows of one block when
 // bs >= 64, or 64 / bs boxes of bs rows when bs is 16 or 32.  Every box lands at a multiple of 1024 bytes of the tile
 // (bs >= 16 rows of 128 bytes), so the 128-byte swizzle of the pieces equals that of one 64-row box.
@@ -154,9 +155,8 @@ paged_prefill_sm90_kernel(const __grid_constant__ CUtensorMap tq, const __grid_c
     mma_ss_64<DP>(&sc[0][0], q_addr, kAtomRows64, sk, kAtomRows64);
     mma_sync_all();
 
-    // causal mask + online softmax (rows g and g + 8 of this warp; a quad of lanes shares a row)
+    // scale to exp2 and mask: key j is visible to query position p iff j <= p
     const bool need_mask = kv0 + kTile - 1 > shift + row0;
-    float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int n = 0; n < 8; ++n) {
 #pragma unroll
@@ -164,43 +164,9 @@ paged_prefill_sm90_kernel(const __grid_constant__ CUtensorMap tq, const __grid_c
         float v = sc[n][e] * scale_log2;
         if (need_mask && kv0 + n * 8 + 2 * t + (e & 1) > qpos[e >> 1]) v = -INFINITY;
         sc[n][e] = v;
-        mx[e >> 1] = fmaxf(mx[e >> 1], v);
       }
     }
-    float corr[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-      const float m_new = fmaxf(m_r[r], mx[r]);
-      corr[r] = m_new == -INFINITY ? 1.f : ex2_approx(m_r[r] - m_new);
-      m_r[r] = m_new;
-      l_r[r] *= corr[r];
-    }
-    uint32_t pf[4][4];  // P as the register A operand of P V: k16 block kk = score columns [16 kk, 16 kk + 16)
-#pragma unroll
-    for (int n = 0; n < 8; ++n) {
-      float p[4];
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float m = m_r[e >> 1];
-        p[e] = m == -INFINITY ? 0.f : ex2_approx(sc[n][e] - m);
-      }
-      l_r[0] += p[0] + p[1];
-      l_r[1] += p[2] + p[3];
-      pf[n >> 1][(n & 1) * 2 + 0] = pack_bf16x2(p[0], p[1]);
-      pf[n >> 1][(n & 1) * 2 + 1] = pack_bf16x2(p[2], p[3]);
-    }
-#pragma unroll
-    for (int i = 0; i < DP / 8; ++i) {
-      o[i][0] *= corr[0];
-      o[i][1] *= corr[0];
-      o[i][2] *= corr[1];
-      o[i][3] *= corr[1];
-    }
-    wgmma_fence();
-    mma_rs<DP>(&o[0][0], pf, sv, kAtomRows64);  // O += P V
-    mma_sync_all();
+    fwd_softmax_pv<DP>(sc, o, m_r, l_r, sv);
     __syncthreads();  // the warpgroup is done with stage s: refill it with tile j + 2
     if (threadIdx.x == 0 && j + 2 < n_tiles) issue_kv(j + 2);
   }
