@@ -247,7 +247,17 @@ class DecoderLM:
         dev = self.device
         r, tp = self.rank, self.tp
         self.alibi = None
-        if cfg.arch == "llama":
+        # The families share one transformer block; what differs is chosen here.  Every QKV projection is laid out
+        # (K/V head, {its G query heads, k, v}, D), G = 1 outside Llama.
+        llama = cfg.arch == "llama"
+        self.G = nh // cfg.kv_heads
+        self._split_qkv = self._split_rope if llama else self._split_rotary if cfg.rotary_dim else self._split
+        self._mlp = self._mlp_swiglu if llama else self._mlp_act
+        self._decode_attention = self._decode_attention_gqa if llama else self._decode_attention_mha
+        # Llama's LM head runs the weight-streaming GEMV for 8 rows or fewer (a prefill's last tokens), the OPT
+        # family's always the GEMM
+        self.head_gemv = llama
+        if llama:
             self._init_llama(params, rnd, fp8)
             return
         wte = get("embed_tokens", V, H)
@@ -256,8 +266,11 @@ class DecoderLM:
         self.pos_offset = 2 if cfg.arch == "opt" else 0
         self.wpe = get("embed_positions", cfg.max_position_embeddings + self.pos_offset, H).to(dev) \
             if cfg.arch == "opt" else None
-        self.emb_ln = (get("emb_ln.g", H, ones=True).to(dev), get("emb_ln.b", H, zeros=True).to(dev)) \
-            if cfg.arch == "bloom" else None
+
+        def ln(name):                     # (gamma, beta, eps): what norm_rows and the decode GEMV's prologue take
+            return get(name + ".g", H, ones=True).to(dev), get(name + ".b", H, zeros=True).to(dev), cfg.layer_norm_eps
+
+        self.emb_ln = ln("emb_ln") if cfg.arch == "bloom" else None
         self.layers: List[Dict] = []
         hl = self.nh_local * self.D
         for i in range(cfg.num_hidden_layers):
@@ -272,14 +285,14 @@ class DecoderLM:
             fc1_b = get(p + "fc1.b", I, zeros=True)[r * (I // tp):(r + 1) * (I // tp)]
             fc2_w = get(p + "fc2.w", H, I)[:, r * (I // tp):(r + 1) * (I // tp)]
             self.layers.append({
-                "ln1": (get(p + "ln1.g", H, ones=True).to(dev), get(p + "ln1.b", H, zeros=True).to(dev)),
-                "ln2": (get(p + "ln2.g", H, ones=True).to(dev), get(p + "ln2.b", H, zeros=True).to(dev)),
+                "ln1": ln(p + "ln1"),
+                "ln2": ln(p + "ln2"),
                 "qkv": _TPLinear(qkv_w.contiguous().to(dev), qkv_b.contiguous().to(dev), fp8),
                 "out": _TPLinear(out_w.contiguous().to(dev), get(p + "out.b", H, zeros=True).to(dev) if r == 0 else None, fp8),
                 "fc1": _TPLinear(fc1_w.contiguous().to(dev), fc1_b.contiguous().to(dev), fp8),
                 "fc2": _TPLinear(fc2_w.contiguous().to(dev), get(p + "fc2.b", H, zeros=True).to(dev) if r == 0 else None, fp8),
             })
-        self.final_ln = (get("final_ln.g", H, ones=True).to(dev), get("final_ln.b", H, zeros=True).to(dev))
+        self.final_ln = ln("final_ln")
         if cfg.tie_word_embeddings:
             self.head_w, self.head_b = self.wte, None
         else:                                                          # vocab-parallel like the embedding
@@ -294,8 +307,7 @@ class DecoderLM:
         (K/V head, {G query heads, k, v}, D) and the interleaved (gate, up) rows of fc1 split by columns, the
         out-projection and fc2 by rows, the embedding and head by vocabulary."""
         cfg, dev, r, tp = self.cfg, self.device, self.rank, self.tp
-        H, I, V, D = cfg.hidden_size, cfg.ffn_dim, cfg.vocab_size, self.D
-        G = cfg.num_attention_heads // cfg.kv_heads
+        H, I, V, D, G = cfg.hidden_size, cfg.ffn_dim, cfg.vocab_size, self.D, self.G
         std = 0.02
 
         def get(name, *shape, ones=False):
@@ -433,12 +445,22 @@ class DecoderLM:
         if self.wpe is not None:
             x = x + ops.fast.embedding(position_ids + self.pos_offset, self.wpe)
         if self.emb_ln is not None:
-            x = ops.fast.layer_norm(x, self.emb_ln[0], self.emb_ln[1], self.cfg.layer_norm_eps)[0]
+            x = ops.fast.norm_rows(x, self.emb_ln)
         return x
 
-    def _rotary(self, q, k, position_ids):
+    # ---- the per-family pieces of the block, chosen in __init__
+    def _split(self, qkv, position_ids):
+        """q [B, T, kv_local, G, D], k / v [B, T, kv_local, D]: views of the projection qkv [B, T, kv_local, G + 2, D].
+        No rotary."""
+        G = self.G
+        return qkv[:, :, :, :G], qkv[:, :, :, G], qkv[:, :, :, G + 1]
+
+    def _split_rotary(self, qkv, position_ids):
+        """`_split` with CodeGen's partial rotary (G = 1): the first rotary_dim channels of q and k rotated as
+        interleaved pairs."""
+        q, k, v = self._split(qkv, position_ids)
         rd = self.cfg.rotary_dim
-        inv = 1.0 / (10000 ** (torch.arange(0, rd, 2, device=q.device, dtype=torch.float32) / rd))
+        inv = 1.0 / (10000 ** (torch.arange(0, rd, 2, device=qkv.device, dtype=torch.float32) / rd))
         ang = position_ids[..., None].float() * inv            # [B, S, rd/2]
         sin, cos = ang.sin()[:, :, None, :], ang.cos()[:, :, None, :]
 
@@ -446,126 +468,95 @@ class DecoderLM:
             t1, t2 = t[..., :rd:2].float(), t[..., 1:rd:2].float()
             out = torch.stack([t1 * cos - t2 * sin, t2 * cos + t1 * sin], dim=-1).flatten(-2)
             return torch.cat([out.to(t.dtype), t[..., rd:]], dim=-1)
-        return rot(q), rot(k)
+        return rot(q[:, :, :, 0])[:, :, :, None], rot(k), v
+
+    def _split_rope(self, qkv, position_ids):
+        """`_split` with Llama's rotary: the query heads and k rotated in one kernel on the packed tensor."""
+        return self._split(ops.fast.rotary_packed(qkv, position_ids, self.cfg.rope_theta, False), position_ids)
+
+    def _mlp_act(self, l, h, ln=None, residual=None):
+        return l["fc2"](l["fc1"](h, self.cfg.activation, ln=ln), residual=residual)
+
+    def _mlp_swiglu(self, l, h, ln=None, residual=None):
+        gu = l["fc1"](h, ln=ln)                                 # (gate, up) pairs interleaved
+        return l["fc2"](ops.fast.swiglu(gu.view(*gu.shape[:-1], -1, 2)), residual=residual)
+
+    def _decode_attention_mha(self, qkv, kc, vc, kv_len, position_ids, scale):
+        q, k, v = self._split_qkv(qkv, position_ids)
+        return ops.fast.decode_attention(q[:, :, :, 0], k, v, kc, vc, kv_len, scale)
+
+    def _decode_attention_gqa(self, qkv, kc, vc, kv_len, position_ids, scale):
+        return ops.fast.decode_attention_gqa(qkv, kc, vc, kv_len, position_ids, scale, self.cfg.rope_theta)
+
+    def _head(self, x):
+        """This rank's vocabulary shard of the logits of the last hidden states x [.., H]: final norm, LM head."""
+        x = ops.fast.norm_rows(x.contiguous(), self.final_ln)
+        if self.head_gemv and x.numel() // x.shape[-1] <= 8:
+            return ops.fast.linear_decode(x, self.head_w, None)
+        return ops.fast.linear(x, self.head_w, self.head_b)
+
+    def _layers(self, x, position_ids, cache, attend):
+        """The transformer blocks over x [B, T, H].  `attend(q, k, v, kc, vc)` writes a layer's new K/V to its cache
+        and returns the attention output of q [B, T, kv_local, G, D]."""
+        B, T = x.shape[:2]
+        for l, (kc, vc) in zip(self.layers, cache):
+            h = ops.fast.norm_rows(x, l["ln1"])
+            q, k, v = self._split_qkv(l["qkv"](h).view(B, T, self.kv_local, self.G + 2, self.D), position_ids)
+            a = l["out"](attend(q, k, v, kc, vc).reshape(B, T, self.nh_local * self.D))
+            if self.cfg.parallel_block:             # x + attn(ln(x)) + mlp(ln(x)): one all-reduce for both branches
+                x = x + self._all_reduce(a + self._mlp(l, h))
+                continue
+            x = x + self._all_reduce(a)
+            x = x + self._all_reduce(self._mlp(l, ops.fast.norm_rows(x, l["ln2"])))
+        return x
 
     def forward(self, input_ids: torch.Tensor, position_ids: torch.Tensor, cache, cache_len: int,
                 last_only: bool = True) -> torch.Tensor:
         """Run `input_ids` [B, T] whose first token sits at sequence position `cache_len`; appends K/V to the cache.
         Returns logits [B, 1 or T, V_local] (this rank's vocabulary shard)."""
-        cfg = self.cfg
-        B, T = input_ids.shape
-        x = self._embed(input_ids, position_ids)
         scale = 1.0 / math.sqrt(self.D)
-        end = cache_len + T
-        if cfg.arch == "llama":
-            return self._forward_llama(x, position_ids, cache, cache_len, last_only)
-        for l, (kc, vc) in zip(self.layers, cache):
-            h = ops.fast.layer_norm(x, l["ln1"][0], l["ln1"][1], cfg.layer_norm_eps)[0]
-            qkv = l["qkv"](h).view(B, T, self.nh_local, 3, self.D)
-            q, k, v = qkv[:, :, :, 0], qkv[:, :, :, 1], qkv[:, :, :, 2]
-            if cfg.rotary_dim:
-                q, k = self._rotary(q, k, position_ids)
+        end = cache_len + input_ids.shape[1]
+
+        def attend(q, k, v, kc, vc):
             self._cache_write(kc, vc, k, v, cache_len)
             kk, vv = self._cache_read(kc, vc, end)
-            if self.alibi is None:
-                o, _ = ops.fast.attention(q if q.stride(-1) == 1 else q.contiguous(), kk, vv, scale, True)
-            else:
-                o = self._attention_alibi(q, kk, vv, scale, cache_len)
-            a = l["out"](o.reshape(B, T, self.nh_local * self.D))
-            if cfg.parallel_block:                  # x + attn(ln(x)) + mlp(ln(x)): one all-reduce for both branches
-                x = x + self._all_reduce(a + l["fc2"](l["fc1"](h, cfg.activation)))
-                continue
-            x = x + self._all_reduce(a)
-            h = ops.fast.layer_norm(x, l["ln2"][0], l["ln2"][1], cfg.layer_norm_eps)[0]
-            m = self._all_reduce(l["fc2"](l["fc1"](h, cfg.activation)))
-            x = x + m
-        if last_only:
-            x = x[:, -1:]
-        x = ops.fast.layer_norm(x.contiguous(), self.final_ln[0], self.final_ln[1], cfg.layer_norm_eps)[0]
-        return ops.fast.linear(x, self.head_w, self.head_b)
-
-    def _mlp_llama(self, l, h):
-        gu = l["fc1"](h)
-        return l["fc2"](ops.fast.swiglu(gu.view(*gu.shape[:-1], gu.shape[-1] // 2, 2)))
-
-    def _forward_llama(self, x, position_ids, cache, cache_len, last_only):
-        cfg = self.cfg
-        B, T = x.shape[:2]
-        G = cfg.num_attention_heads // cfg.kv_heads
-        scale = 1.0 / math.sqrt(self.D)
-        end = cache_len + T
-        for l, (kc, vc) in zip(self.layers, cache):
-            h = ops.fast.norm_rows(x, l["ln1"])
-            qkv = l["qkv"](h).view(B, T, self.kv_local, G + 2, self.D)
-            qkv = ops.fast.rotary_packed(qkv, position_ids, cfg.rope_theta, False)
-            self._cache_write(kc, vc, qkv[:, :, :, G], qkv[:, :, :, G + 1], cache_len)
+            if self.alibi is not None:
+                return self._attention_alibi(q[:, :, :, 0], kk, vv, scale, cache_len)
             # the grouped Q view against the valid cache rows: causal with Sq != Sk
-            o, _ = ops.fast.attention(qkv[:, :, :, :G], *self._cache_read(kc, vc, end), scale, True)
-            x = x + self._all_reduce(l["out"](o.reshape(B, T, self.nh_local * self.D)))
-            x = x + self._all_reduce(self._mlp_llama(l, ops.fast.norm_rows(x, l["ln2"])))
-        if last_only:
-            x = x[:, -1:]
-        return self._head_llama(ops.fast.norm_rows(x.contiguous(), self.final_ln))
+            return ops.fast.attention(q, kk, vv, scale, True)[0]
 
-    def _head_llama(self, x):
-        """The LM head: the weight-streaming GEMV for the few rows of a prefill's last tokens, else the GEMM."""
-        if x.numel() // x.shape[-1] <= 8:
-            return ops.fast.linear_decode(x, self.head_w, None)
-        return ops.fast.linear(x, self.head_w, None)
+        x = self._layers(self._embed(input_ids, position_ids), position_ids, cache, attend)
+        return self._head(x[:, -1:] if last_only else x)
 
     def decode_step(self, input_ids: torch.Tensor, position_ids: torch.Tensor, cache, kv_len: torch.Tensor) -> torch.Tensor:
         """One new token per sequence with every position-dependent quantity on the device: `position_ids` [B, 1]
         (int64) is both the embedding position and the cache row to write, `kv_len` (int32 scalar tensor) the number
         of valid cache rows afterwards.  Shapes never change, so the step can be replayed from one CUDA graph.
         Returns logits [B, 1, V_local]."""
-        cfg = self.cfg
         assert self.alibi is None, "graph decode is implemented for learned / rotary position models"
         B = input_ids.shape[0]
         x = self._embed(input_ids, position_ids)
         scale = 1.0 / math.sqrt(self.D)
-        eps = cfg.layer_norm_eps
-        if cfg.arch == "llama":
-            G = cfg.num_attention_heads // cfg.kv_heads
-            for l, (kc, vc) in zip(self.layers, cache):
-                # 5 launches per layer (7 under tensor parallelism): RMSNorm in the QKV / fc1 GEMV prologues, rotary and
-                # the cache append in the attention kernel, residual adds in the GEMV / all-reduce epilogues
-                qkv = l["qkv"](x, ln=l["ln1"]).view(B, 1, self.kv_local, G + 2, self.D)
-                o = ops.fast.decode_attention_gqa(qkv, kc, vc, kv_len, position_ids, scale, cfg.rope_theta)
-                o = o.reshape(B, 1, self.nh_local * self.D)
-                if self.tp == 1:
-                    x = l["out"](o, residual=x)
-                    gu = l["fc1"](x, ln=l["ln2"])
-                    x = l["fc2"](ops.fast.swiglu(gu.view(B, 1, -1, 2)), residual=x)
-                else:
-                    x = self._all_reduce(l["out"](o), residual=x)
-                    gu = l["fc1"](x, ln=l["ln2"])
-                    x = self._all_reduce(l["fc2"](ops.fast.swiglu(gu.view(B, 1, -1, 2))), residual=x)
-            return ops.fast.linear_decode(x.contiguous(), self.head_w, None, None, ln=self.final_ln)
         for l, (kc, vc) in zip(self.layers, cache):
-            # 5 launches per layer (7 under tensor parallelism): LN rides in the GEMV prologues, the cache append in
-            # the attention kernel, residual adds in the GEMV / all-reduce epilogues
-            qkv = l["qkv"](x, ln=(l["ln1"][0], l["ln1"][1], eps)).view(B, 1, self.nh_local, 3, self.D)
-            q, k, v = qkv[:, :, :, 0], qkv[:, :, :, 1], qkv[:, :, :, 2]
-            if cfg.rotary_dim:
-                q, k = self._rotary(q, k, position_ids)
-            o = ops.fast.decode_attention(q, k, v, kc, vc, kv_len, scale).reshape(B, 1, self.nh_local * self.D)
-            if cfg.parallel_block:
+            # 5 launches per layer, 6 with Llama's SwiGLU (2 more under tensor parallelism): the norms ride in the GEMV
+            # prologues, the cache append (and Llama's rotary) in the attention kernel, residual adds in the GEMV /
+            # all-reduce epilogues
+            qkv = l["qkv"](x, ln=l["ln1"]).view(B, 1, self.kv_local, self.G + 2, self.D)
+            o = self._decode_attention(qkv, kc, vc, kv_len, position_ids, scale).reshape(B, 1, self.nh_local * self.D)
+            if self.cfg.parallel_block:
                 # both branches read LN1(x) (recomputed in the second GEMV's prologue); the MLP branch rides in as the
                 # residual of the out-projection, the block input as the residual of the last GEMV / the all-reduce
-                m = l["fc2"](l["fc1"](x, cfg.activation, ln=(l["ln1"][0], l["ln1"][1], eps)),
-                             residual=x if self.tp == 1 else None)
+                m = self._mlp(l, x, ln=l["ln1"], residual=x if self.tp == 1 else None)
                 x = l["out"](o, residual=m) if self.tp == 1 else self._all_reduce(l["out"](o, residual=m), residual=x)
                 continue
             if self.tp == 1:
                 x = l["out"](o, residual=x)
-                x = l["fc2"](l["fc1"](x, cfg.activation, ln=(l["ln2"][0], l["ln2"][1], eps)), residual=x)
+                x = self._mlp(l, x, ln=l["ln2"], residual=x)
             else:
                 x = self._all_reduce(l["out"](o), residual=x)
-                x = self._all_reduce(l["fc2"](l["fc1"](x, cfg.activation, ln=(l["ln2"][0], l["ln2"][1], eps))),
-                                     residual=x)
-        # LM head: 257 MB of bf16 weights streamed once per token, final LN in the prologue
-        return ops.fast.linear_decode(x.contiguous(), self.head_w, None, self.head_b,
-                                      ln=(self.final_ln[0], self.final_ln[1], eps))
+                x = self._all_reduce(self._mlp(l, x, ln=l["ln2"]), residual=x)
+        # LM head: this rank's vocabulary shard of the weights streamed once per token, final norm in the prologue
+        return ops.fast.linear_decode(x.contiguous(), self.head_w, None, self.head_b, ln=self.final_ln)
 
     # ------------------------------------------------------------------ ragged 1-D batches (iteration-level batching)
     def init_cache_1d(self, num_slots: int):
@@ -590,62 +581,32 @@ class DecoderLM:
         `ops.ragged_attention`.
         Returns logits [len(logit_index), V_local] of the rows in `logit_index` (the last token of every sequence).
         (reference: OPTForLMModule.__call__ of opt_model_1d.py:378 with fused_mmha)"""
-        cfg = self.cfg
         T = input_ids.shape[0]
-        x = self._embed(input_ids.view(1, T), position.view(1, T))[0]          # [T, H]
         scale = 1.0 / math.sqrt(self.D)
         alibi = self.alibi.float().contiguous() if self.alibi is not None else None
         if chunks is not None and alibi is not None:
             raise ValueError("the paged prefill kernel takes no ALiBi")
 
-        def attend(q, kc, vc, q_pre=None):
-            # q [T, h, D] (q_pre: a view of its prefill rows the kernel can read in place, e.g. the grouped projection)
+        def attend(q, k, v, kc, vc):
+            self._cache_write(kc, vc, k, v, slot)
+            # the ragged kernel takes q as [T, heads, D] (a copy when G > 1), the prefill kernel reads the grouped view
+            qh = q.reshape(T, self.nh_local, self.D)
             if chunks is None or n_prefill == 0:
-                return ops.fast.ragged_attention(q, kc, vc, seq_start, ctx_len, scale, max_ctx, alibi, block_table,
+                return ops.fast.ragged_attention(qh, kc, vc, seq_start, ctx_len, scale, max_ctx, alibi, block_table,
                                                  block_size)
-            o = ops.fast.paged_prefill_attention(q[:n_prefill] if q_pre is None else q_pre, kc, vc, block_table,
-                                                 block_size, *chunks, scale, max_ctx)
+            o = ops.fast.paged_prefill_attention(q[0, :n_prefill], kc, vc, block_table, block_size, *chunks, scale,
+                                                 max_ctx)
             if n_prefill == T:
                 return o
-            r = ops.fast.ragged_attention(q[n_prefill:], kc, vc, seq_start[n_prefill:], ctx_len[n_prefill:], scale,
+            r = ops.fast.ragged_attention(qh[n_prefill:], kc, vc, seq_start[n_prefill:], ctx_len[n_prefill:], scale,
                                           max_ctx, None, block_table, block_size)
             return torch.cat([o, r])
 
-        if cfg.arch == "llama":
-            G = cfg.num_attention_heads // cfg.kv_heads
-            for l, (kc, vc) in zip(self.layers, cache):
-                qkv = l["qkv"](ops.fast.norm_rows(x, l["ln1"])).view(1, T, self.kv_local, G + 2, self.D)
-                qkv = ops.fast.rotary_packed(qkv, position.view(1, T), cfg.rope_theta, False)[0]
-                self._cache_write(kc, vc, qkv[None, :, :, G], qkv[None, :, :, G + 1], slot)
-                q = qkv[:, :, :G].reshape(T, self.nh_local, self.D)
-                o = attend(q, kc, vc, qkv[:n_prefill, :, :G])
-                x = x + self._all_reduce(l["out"](o.reshape(T, self.nh_local * self.D)))
-                x = x + self._all_reduce(self._mlp_llama(l, ops.fast.norm_rows(x, l["ln2"])))
-            if logit_index.numel() == 0:
-                return x.new_empty(0, self.V_local)
-            return self._head_llama(ops.fast.norm_rows(x.index_select(0, logit_index).contiguous(), self.final_ln))
-        for l, (kc, vc) in zip(self.layers, cache):
-            h = ops.fast.layer_norm(x, l["ln1"][0], l["ln1"][1], cfg.layer_norm_eps)[0]
-            qkv = l["qkv"](h).view(T, self.nh_local, 3, self.D)
-            q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
-            if cfg.rotary_dim:
-                q, k = self._rotary(q[None], k[None], position.view(1, T))
-                q, k = q[0], k[0]
-            self._cache_write(kc, vc, k[None], v[None], slot)
-            o = attend(q, kc, vc)
-            a = l["out"](o.reshape(T, self.nh_local * self.D))
-            if cfg.parallel_block:
-                x = x + self._all_reduce(a + l["fc2"](l["fc1"](h, cfg.activation)))
-                continue
-            x = x + self._all_reduce(a)
-            h = ops.fast.layer_norm(x, l["ln2"][0], l["ln2"][1], cfg.layer_norm_eps)[0]
-            m = self._all_reduce(l["fc2"](l["fc1"](h, cfg.activation)))
-            x = x + m
+        # one batch row of T tokens
+        x = self._layers(self._embed(input_ids.view(1, T), position.view(1, T)), position.view(1, T), cache, attend)
         if logit_index.numel() == 0:
             return x.new_empty(0, self.V_local)
-        x = x.index_select(0, logit_index)
-        x = ops.fast.layer_norm(x.contiguous(), self.final_ln[0], self.final_ln[1], cfg.layer_norm_eps)[0]
-        return ops.fast.linear(x, self.head_w, self.head_b)
+        return self._head(x[0].index_select(0, logit_index))
 
     def _attention_alibi(self, q, k, v, scale, cache_len):
         B, T, h, D = q.shape

@@ -1332,10 +1332,11 @@ class RMSNormArgs(NamedTuple):
 
 
 def norm_rows(x: Tensor, ln: Union[Tuple[Tensor, Tensor, float], RMSNormArgs]) -> Tensor:
-    """x normalised by `ln`: a LayerNorm (gamma, beta, eps) or an RMSNormArgs."""
+    """x normalised by `ln`: a LayerNorm (gamma, beta, eps) or an RMSNormArgs.  Not differentiable: like every `fast`
+    entry point it calls the implementations directly, not through the dispatcher."""
     if isinstance(ln, RMSNormArgs):
-        return rms_norm(x, ln.gamma, ln.eps)[0]
-    return layer_norm(x, ln[0], ln[1], ln[2])[0]
+        return rms_norm._init_fn(x, ln.gamma, ln.eps)[0]
+    return layer_norm._init_fn(x, ln[0], ln[1], ln[2])[0]
 
 
 def linear_decode(x: Tensor, w: Tensor, w_scale: Optional[Tensor], b: Optional[Tensor] = None, act: str = "none",
