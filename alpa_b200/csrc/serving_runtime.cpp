@@ -202,6 +202,9 @@ class KVCacheManager {
 // block before its length, so no shared or indexed row is ever handed out as a write slot (prepare_inputs checks it).
 // Allocation takes uncached free blocks first (lowest index), then evicts cached blocks, least recently released first
 // (a sequence releases its blocks last one first).
+// A sequence's `namespace` (allocate / match_prefix) is the root of its chain: blocks are shared only between sequences
+// of one namespace.  K/V depend on more than the tokens when a LoRA adapter is applied, so the pool passes the adapter's
+// load id (never reused); namespace 0 is the base model and keeps the keys of a manager without namespaces.
 class PagedKVCacheManager {
  public:
   PagedKVCacheManager(int64_t num_blocks, int64_t block_size, bool prefix_caching = false, int hash_bits = 64)
@@ -236,9 +239,10 @@ class PagedKVCacheManager {
     return entries_[block].id != 0;
   }
 
-  void allocate(int64_t seq_id) {
+  void allocate(int64_t seq_id, int64_t ns = 0) {
     if (seqs_.count(seq_id)) throw std::invalid_argument("sequence " + std::to_string(seq_id) + " is already allocated");
-    seqs_[seq_id];
+    const uint64_t root = chain_root(ns);
+    seqs_[seq_id].chain = root;
   }
 
   void release(int64_t seq_id) {
@@ -262,13 +266,13 @@ class PagedKVCacheManager {
   // Allocate `seq_id` with the longest chain of indexed blocks matching `token_ids`, taking a reference on each.
   // Returns the tokens hit: a multiple of block_size, at most ((len(token_ids) - 1) / block_size) * block_size so the
   // last token is always computed (its logits are needed, and it never writes into a shared block).
-  int64_t match_prefix(int64_t seq_id, const std::vector<int64_t>& token_ids) {
+  int64_t match_prefix(int64_t seq_id, const std::vector<int64_t>& token_ids, int64_t ns = 0) {
     if (!prefix_caching_) throw std::invalid_argument("match_prefix needs a manager with prefix_caching=True");
     if (seqs_.count(seq_id)) throw std::invalid_argument("sequence " + std::to_string(seq_id) + " is already allocated");
     const int64_t n = static_cast<int64_t>(token_ids.size());
     const int64_t max_blocks = n > 0 ? (n - 1) / block_size_ : 0;
     std::vector<int32_t> hit;
-    uint64_t parent = 0;
+    uint64_t parent = chain_root(ns);
     for (int64_t k = 0; k < max_blocks; ++k) {
       const int32_t b = lookup(parent, token_ids.data() + k * block_size_);
       if (b < 0) break;
@@ -422,7 +426,7 @@ class PagedKVCacheManager {
     std::vector<int32_t> blocks;
     int64_t length = 0;           // tokens written
     std::vector<int64_t> tokens;  // token ids of positions [0, tokens.size()) (prefix caching)
-    uint64_t chain = 0;           // index entry of the prefix made of blocks [0, chained); 0 = the empty prefix
+    uint64_t chain = 0;           // index entry of the prefix made of blocks [0, chained), or the namespace's root
     int64_t chained = 0;
   };
   struct Entry {
@@ -431,6 +435,13 @@ class PagedKVCacheManager {
     uint64_t hash = 0;
     std::vector<int64_t> tokens;
   };
+
+  // The parent key of a namespace's first block.  Entry ids count up from 1 and never reach bit 63, so a root of
+  // namespace > 0 is never an entry id; namespace 0 keeps the root 0.
+  static uint64_t chain_root(int64_t ns) {
+    if (ns < 0) throw std::invalid_argument("prefix cache namespace must be >= 0");
+    return ns == 0 ? 0 : (uint64_t{1} << 63) | static_cast<uint64_t>(ns);
+  }
 
   PagedSeq& get(int64_t seq_id) {
     auto it = seqs_.find(seq_id);
@@ -562,7 +573,7 @@ void bind_serving_runtime(py::module_& m) {
       .def_property_readonly("num_free_blocks", &PagedKVCacheManager::num_free_blocks)
       .def_property_readonly("num_sequences", &PagedKVCacheManager::num_sequences)
       .def("has", &PagedKVCacheManager::has)
-      .def("allocate", &PagedKVCacheManager::allocate)
+      .def("allocate", &PagedKVCacheManager::allocate, py::arg("seq_id"), py::arg("namespace") = 0)
       .def("free", &PagedKVCacheManager::release)
       .def("append", &PagedKVCacheManager::append)
       .def("blocks_needed", &PagedKVCacheManager::blocks_needed)
@@ -573,7 +584,8 @@ void bind_serving_runtime(py::module_& m) {
       .def_property_readonly("num_evictable_blocks", &PagedKVCacheManager::num_evictable_blocks)
       .def("ref_count", &PagedKVCacheManager::ref_count)
       .def("is_cached", &PagedKVCacheManager::is_cached)
-      .def("match_prefix", &PagedKVCacheManager::match_prefix, py::arg("seq_id"), py::arg("token_ids"))
+      .def("match_prefix", &PagedKVCacheManager::match_prefix, py::arg("seq_id"), py::arg("token_ids"),
+           py::arg("namespace") = 0)
       .def("reset_prefix_cache", &PagedKVCacheManager::reset_prefix_cache)
       .def("prepare_inputs", &PagedKVCacheManager::prepare_inputs, py::arg("prefill_ids"), py::arg("prefill_lens"),
            py::arg("decode_ids"), py::arg("batch_tokens"), py::arg("pad_slot"),

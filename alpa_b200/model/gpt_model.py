@@ -300,27 +300,34 @@ def llama_config_from_hf(hf_config, **kw) -> GPTConfig:
     return GPTConfig(**args)
 
 
+def pack_llama_qkv(q, k, v, kv_heads: int):
+    """The fused QKV rows: for each K/V head, the q rows of its G query heads, then its k rows, then its v rows.
+    q: [heads * D, X], k / v: [kv_heads * D, X], for any row width X (a weight, or a LoRA B)."""
+    X = q.shape[-1]
+    return torch.cat([t.reshape(kv_heads, -1, X) for t in (q, k, v)], 1).reshape(-1, X)
+
+
+def pack_llama_fc1(gate, up):
+    """fc1's rows: gate_proj and up_proj rows interleaved.  gate / up: [I, X] -> [2 I, X]."""
+    return torch.stack([gate, up], 1).reshape(2 * gate.shape[0], gate.shape[-1])
+
+
 def llama_params_from_hf(state_dict, cfg: GPTConfig) -> dict:
     """GPTModel(cfg) parameters (arch="llama", cast to cfg.dtype) from a LlamaForCausalLM state dict.  The fused QKV
     weight takes, for each K/V head, the q_proj rows of its G query heads, then its k_proj rows, then its v_proj rows;
     fc1 interleaves gate_proj and up_proj rows."""
     sd = {k[len("model."):] if k.startswith("model.") else k: v for k, v in state_dict.items()}
-    H, nh = cfg.hidden_size, cfg.num_attention_heads
-    kv, D, I = cfg.num_key_value_heads or nh, H // nh, cfg.intermediate_size
-    G = nh // kv
+    kv = cfg.num_key_value_heads or cfg.num_attention_heads
     out = {"wte": sd["embed_tokens.weight"], "ln_f_g": sd["norm.weight"]}
     if not cfg.tie_word_embeddings:
         out["decoder_w"] = sd["lm_head.weight"]
     for i in range(cfg.num_hidden_layers):
         p, a, m = f"layers.{i}.", f"layers.{i}.self_attn.", f"layers.{i}.mlp."
-        q = sd[a + "q_proj.weight"].reshape(kv, G, D, H)
-        k = sd[a + "k_proj.weight"].reshape(kv, 1, D, H)
-        v = sd[a + "v_proj.weight"].reshape(kv, 1, D, H)
         b = f"blocks.{i}."
-        out[b + "qkv_w"] = torch.cat([q, k, v], 1).reshape(-1, H)
+        out[b + "qkv_w"] = pack_llama_qkv(sd[a + "q_proj.weight"], sd[a + "k_proj.weight"], sd[a + "v_proj.weight"], kv)
         out[b + "proj_w"] = sd[a + "o_proj.weight"]
         out[b + "ln1_g"] = sd[p + "input_layernorm.weight"]
         out[b + "ln2_g"] = sd[p + "post_attention_layernorm.weight"]
-        out[b + "fc1_w"] = torch.stack([sd[m + "gate_proj.weight"], sd[m + "up_proj.weight"]], 1).reshape(2 * I, H)
+        out[b + "fc1_w"] = pack_llama_fc1(sd[m + "gate_proj.weight"], sd[m + "up_proj.weight"])
         out[b + "fc2_w"] = sd[m + "down_proj.weight"]
     return {k: v.detach().to(cfg.dtype).contiguous() for k, v in out.items()}

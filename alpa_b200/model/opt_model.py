@@ -21,6 +21,8 @@ for its whole group of query heads.
 from __future__ import annotations
 
 import math
+import re
+import weakref
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Tuple
 
@@ -29,6 +31,7 @@ import torch.distributed as dist
 import torch.nn.functional as F
 
 from alpa_b200 import ops
+from alpa_b200.model.gpt_model import pack_llama_fc1, pack_llama_qkv
 
 
 @dataclass
@@ -57,10 +60,15 @@ class OPTConfig:
     rope_theta: float = 10000.0
     # bf16 | fp8: e4m3 K/V rows with one fp32 scale per (token, K/V head) (ops.Fp8KV), about half the cache bytes
     kv_cache_dtype: str = "bf16"
+    # multi-LoRA serving: adapter slots (0 = off: nothing is allocated) and the largest rank an adapter may have
+    max_loras: int = 0
+    max_lora_rank: int = 16
 
     def __post_init__(self):
         if self.kv_cache_dtype not in ("bf16", "fp8"):
             raise ValueError(f"kv_cache_dtype must be 'bf16' or 'fp8', not {self.kv_cache_dtype!r}")
+        if self.max_loras < 0 or not 1 <= self.max_lora_rank <= 64:
+            raise ValueError("need max_loras >= 0 and 1 <= max_lora_rank <= 64")
         if self.parallel_block is None:
             self.parallel_block = self.arch == "codegen"
         if self.tie_word_embeddings is None:
@@ -192,6 +200,19 @@ class _TPLinear:
         return self.w.numel() * self.w.element_size()
 
 
+# LoRA targets per architecture: the PEFT module name -> (DecoderLM projection, its part of the stacked rank).  OPT's
+# fc1 is no target: its activation is fused into the GEMM epilogue, and the delta would have to go in before it.
+LORA_TARGETS = {
+    "llama": {"q_proj": ("qkv", 0), "k_proj": ("qkv", 1), "v_proj": ("qkv", 2), "o_proj": ("out", 0),
+              "gate_proj": ("fc1", 0), "up_proj": ("fc1", 1), "down_proj": ("fc2", 0)},
+    "opt": {"q_proj": ("qkv", 0), "k_proj": ("qkv", 1), "v_proj": ("qkv", 2), "out_proj": ("out", 0),
+            "fc2": ("fc2", 0)},
+}
+# PEFT tensor names: `base_model.model.model.layers.3.self_attn.q_proj.lora_A.weight`, `...decoder.layers.3.fc2.lora_B
+# .weight`
+_LORA_NAME = re.compile(r"layers\.(\d+)\.(?:\w+\.)?(\w+)\.lora_([AB])(?:\.weight)?$")
+
+
 def _alibi_slopes(n: int) -> torch.Tensor:
     def pow2(k):
         start = 2 ** (-2 ** -(math.log2(k) - 3))
@@ -278,8 +299,7 @@ class DecoderLM:
             qkv_w = get(p + "qkv.w", 3, nh, self.D, H)                  # [(q,k,v), head, D, H]
             # codegen has no attention biases (an all-zero bias is numerically the same and keeps one code path)
             qkv_b = get(p + "qkv.b", 3, nh, self.D, zeros=True)
-            qkv_w = qkv_w[:, r * self.nh_local:(r + 1) * self.nh_local].permute(1, 0, 2, 3).reshape(3 * hl, H)
-            qkv_b = qkv_b[:, r * self.nh_local:(r + 1) * self.nh_local].permute(1, 0, 2).reshape(3 * hl)
+            qkv_w, qkv_b = self._opt_qkv_rows(qkv_w), self._opt_qkv_rows(qkv_b)
             out_w = get(p + "out.w", H, H)[:, r * hl:(r + 1) * hl]
             fc1_w = get(p + "fc1.w", I, H)[r * (I // tp):(r + 1) * (I // tp)]
             fc1_b = get(p + "fc1.b", I, zeros=True)[r * (I // tp):(r + 1) * (I // tp)]
@@ -301,7 +321,13 @@ class DecoderLM:
             self.head_w = hw[r * self.V_local:(r + 1) * self.V_local].contiguous().to(dev)
             self.head_b = hb[r * self.V_local:(r + 1) * self.V_local].contiguous().to(dev)
         self.alibi = _alibi_slopes(nh)[r * self.nh_local:(r + 1) * self.nh_local].to(dev) if cfg.arch == "bloom" else None
+        self._init_lora()
 
+    def _opt_qkv_rows(self, w):
+        """This rank's rows of the OPT-family QKV projection: w [(q, k, v), heads, D, ...] -> [(head, (q, k, v), D), ...]
+        of its heads (a weight, a bias or a LoRA B)."""
+        w = w[:, self.rank * self.nh_local:(self.rank + 1) * self.nh_local]
+        return w.transpose(0, 1).reshape(3 * self.nh_local * self.D, *w.shape[3:])
     def _init_llama(self, params, rnd, fp8):
         """Weights of `GPTModel(arch="llama")` (its state_dict names and layouts), sliced for this rank: the QKV rows
         (K/V head, {G query heads, k, v}, D) and the interleaved (gate, up) rows of fc1 split by columns, the
@@ -340,6 +366,139 @@ class DecoderLM:
         else:
             self.head_w = rows(F.pad(get("decoder_w", V, H), (0, 0, 0, self.Vp - V)), self.V_local)
         self.head_b = None
+        self._init_lora()
+
+    # ------------------------------------------------------------------ LoRA adapters
+    def _init_lora(self):
+        """Stacked adapter tables, per layer and targeted projection: A [slots, R, K_local] and B [slots, N_local, R],
+        zero in unused slots; fused projections stack their parts along R (each part rp rows: max_lora_rank rounded up
+        to 8, ranks below it zero-padded), and B is block-diagonal over them."""
+        cfg = self.cfg
+        self.loras: Dict[str, Tuple[int, int]] = {}          # name -> (slot, load id)
+        self.lora_slot_of: Dict[int, int] = {}               # load id -> slot
+        self._lora_next_id = 1                               # load ids are never reused; 0 is the base model
+        self._lora_pools = weakref.WeakSet()                 # pools whose prompts may use an adapter
+        self.lora_rank_stride = rp = -(-cfg.max_lora_rank // 8) * 8
+        if cfg.max_loras == 0 or cfg.arch not in LORA_TARGETS:
+            return
+        n, dt, dev = cfg.max_loras, cfg.dtype, self.device
+        H, hl, il = cfg.hidden_size, self.nh_local * self.D, cfg.ffn_dim // self.tp
+        # projection -> (N_local, K_local, stacked parts)
+        shapes = {"qkv": (self.kv_local * (self.G + 2) * self.D, H, 3), "out": (H, hl, 1), "fc2": (H, il, 1)}
+        if cfg.arch == "llama":
+            shapes["fc1"] = (2 * il, H, 2)
+        for l in self.layers:
+            l["lora"] = {proj: (torch.zeros(n, k * rp, K, dtype=dt, device=dev),
+                                torch.zeros(n, N, k * rp, dtype=dt, device=dev)) for proj, (N, K, k) in shapes.items()}
+        self.lora_scale = torch.zeros(n, dtype=torch.float32, device=dev)
+
+    def lora_id(self, name: str) -> int:
+        """The load id of a loaded adapter (what `IterationLevelInputPool.enter_prompts(loras=...)` takes)."""
+        if name not in self.loras:
+            raise ValueError(f"unknown LoRA adapter {name!r}")
+        return self.loras[name][1]
+
+    def load_lora(self, name: str, tensors: Dict[str, torch.Tensor], alpha: float, r: int) -> int:
+        """Copy an adapter into a free slot and return the slot.  `tensors`: PEFT names (`...layers.N.self_attn.q_proj.
+        lora_A.weight` [r, in], `...lora_B.weight` [out, r]) of full, unsliced projections; a target it leaves out adds
+        nothing.  The scale is alpha / r.  Raises ValueError when every slot is taken, r exceeds max_lora_rank, the
+        architecture has no LoRA support (only Llama and OPT have) or a tensor is not a supported target of it."""
+        cfg = self.cfg
+        if cfg.arch not in LORA_TARGETS:
+            raise ValueError(f"LoRA adapters are served for Llama and OPT models, not {cfg.arch!r}")
+        if cfg.max_loras == 0:
+            raise ValueError("this model has no LoRA slots (max_loras=0)")
+        if name in self.loras:
+            raise ValueError(f"LoRA adapter {name!r} is already loaded")
+        if not 1 <= int(r) <= cfg.max_lora_rank:
+            raise ValueError(f"LoRA rank {r} is outside 1..max_lora_rank={cfg.max_lora_rank}")
+        used = set(s for s, _ in self.loras.values())
+        free = [s for s in range(cfg.max_loras) if s not in used]
+        if not free:
+            raise ValueError(f"all {cfg.max_loras} LoRA slots are taken")
+        tables = self._lora_tables(tensors, int(r))
+        slot = free[0]
+        for l, t in zip(self.layers, tables):
+            for proj, (A, B) in t.items():
+                l["lora"][proj][0][slot].copy_(A)
+                l["lora"][proj][1][slot].copy_(B)
+        self.lora_scale[slot] = float(alpha) / int(r)
+        lid = self._lora_next_id
+        self._lora_next_id += 1
+        self.loras[name] = (slot, lid)
+        self.lora_slot_of[lid] = slot
+        return slot
+
+    def unload_lora(self, name: str):
+        """Free an adapter's slot.  Raises RuntimeError while a queued or running sequence uses it."""
+        lid = self.lora_id(name)
+        if any(pool.uses_lora(lid) for pool in list(self._lora_pools)):
+            raise RuntimeError(f"LoRA adapter {name!r} is in use by a live sequence")
+        slot, _ = self.loras.pop(name)
+        del self.lora_slot_of[lid]
+        for l in self.layers:
+            for A, B in l["lora"].values():
+                A[slot].zero_()
+                B[slot].zero_()
+        self.lora_scale[slot] = 0.0
+
+    def _lora_tables(self, tensors, r: int):
+        """Per layer, this rank's (A, B) of every projection in the slot layout (see `_init_lora`), built on the CPU."""
+        cfg, rank, tp, rp = self.cfg, self.rank, self.tp, self.lora_rank_stride
+        H, I, D = cfg.hidden_size, cfg.ffn_dim, self.D
+        targets = LORA_TARGETS[cfg.arch]
+        given: List[Dict[str, Dict[str, torch.Tensor]]] = [{} for _ in self.layers]
+        for key, t in tensors.items():
+            m = _LORA_NAME.search(key)
+            if m is None:
+                raise ValueError(f"not a LoRA tensor name: {key!r}")
+            i, mod, ab = int(m.group(1)), m.group(2), m.group(3)
+            if mod not in targets:
+                raise ValueError(f"{mod!r} is not a supported LoRA target of {cfg.arch!r} (supported: "
+                                 f"{sorted(targets)})")
+            if not 0 <= i < len(self.layers):
+                raise ValueError(f"LoRA tensor {key!r}: the model has {len(self.layers)} layers")
+            given[i].setdefault(mod, {})[ab] = torch.as_tensor(t).float()
+        llama = cfg.arch == "llama"
+        dims = {"q_proj": (H, cfg.num_attention_heads * D), "k_proj": (H, cfg.kv_heads * D),
+                "v_proj": (H, cfg.kv_heads * D), "o_proj": (H, H), "out_proj": (H, H), "gate_proj": (H, I),
+                "up_proj": (H, I), "down_proj": (I, H), "fc2": (I, H)}
+        hl, il = self.nh_local * D, I // tp
+        out = []
+        for i, g in enumerate(given):
+            A, B = {}, {}                           # module -> A [rp, in], B [out, rp * parts] in its part's columns
+            for mod, (proj, part) in targets.items():
+                k_in, n_out = dims[mod]
+                parts = 1 + max(p for pj, p in targets.values() if pj == proj)
+                a, b = torch.zeros(rp, k_in), torch.zeros(n_out, parts * rp)
+                if mod in g:
+                    if set(g[mod]) != {"A", "B"}:
+                        raise ValueError(f"layer {i} {mod}: needs both lora_A and lora_B")
+                    ga, gb = g[mod]["A"], g[mod]["B"]
+                    if tuple(ga.shape) != (r, k_in) or tuple(gb.shape) != (n_out, r):
+                        raise ValueError(f"layer {i} {mod}: lora_A {tuple(ga.shape)} / lora_B {tuple(gb.shape)}, "
+                                         f"expected {(r, k_in)} / {(n_out, r)}")
+                    a[:r], b[:, part * rp:part * rp + r] = ga, gb
+                A[mod], B[mod] = a, b
+            t = {}
+            if llama:
+                qkv_local = self.kv_local * (self.G + 2) * D
+                bq = pack_llama_qkv(B["q_proj"], B["k_proj"], B["v_proj"], cfg.kv_heads)
+                t["qkv"] = (torch.cat([A["q_proj"], A["k_proj"], A["v_proj"]]),
+                            bq[rank * qkv_local:(rank + 1) * qkv_local])
+                bf = pack_llama_fc1(B["gate_proj"], B["up_proj"])
+                t["fc1"] = (torch.cat([A["gate_proj"], A["up_proj"]]), bf[rank * 2 * il:(rank + 1) * 2 * il])
+                o, d = "o_proj", "down_proj"
+            else:
+                nh = cfg.num_attention_heads
+                b3 = torch.stack([B[m].view(nh, D, 3 * rp) for m in ("q_proj", "k_proj", "v_proj")])
+                t["qkv"] = (torch.cat([A["q_proj"], A["k_proj"], A["v_proj"]]), self._opt_qkv_rows(b3))
+                o, d = "out_proj", "fc2"
+            # row-parallel layers: A sliced like the weight's columns, B whole
+            t["out"] = (A[o][:, rank * hl:(rank + 1) * hl], B[o])
+            t["fc2"] = (A[d][:, rank * il:(rank + 1) * il], B[d])
+            out.append(t)
+        return out
 
     # ------------------------------------------------------------------ cache
     def _new_kv(self, shape):
@@ -474,12 +633,24 @@ class DecoderLM:
         """`_split` with Llama's rotary: the query heads and k rotated in one kernel on the packed tensor."""
         return self._split(ops.fast.rotary_packed(qkv, position_ids, self.cfg.rope_theta, False), position_ids)
 
-    def _mlp_act(self, l, h, ln=None, residual=None):
-        return l["fc2"](l["fc1"](h, self.cfg.activation, ln=ln), residual=residual)
+    def _mlp_act(self, l, h, ln=None, residual=None, lora=None):
+        z = l["fc1"](h, self.cfg.activation, ln=ln)
+        return self._lora(lora, l, "fc2", z, l["fc2"](z, residual=residual))
 
-    def _mlp_swiglu(self, l, h, ln=None, residual=None):
-        gu = l["fc1"](h, ln=ln)                                 # (gate, up) pairs interleaved
-        return l["fc2"](ops.fast.swiglu(gu.view(*gu.shape[:-1], -1, 2)), residual=residual)
+    def _mlp_swiglu(self, l, h, ln=None, residual=None, lora=None):
+        gu = self._lora(lora, l, "fc1", h, l["fc1"](h, ln=ln))          # (gate, up) pairs interleaved
+        z = ops.fast.swiglu(gu.view(*gu.shape[:-1], -1, 2))
+        return self._lora(lora, l, "fc2", z, l["fc2"](z, residual=residual))
+
+    def _lora(self, lora, l, proj, x, y):
+        """y (the output of projection `proj` for input x, `ln` already applied) plus this rank's LoRA delta of the
+        batch rows that carry an adapter, in place; `lora` = (rows, seg_start, seg_slot) or None (y unchanged)."""
+        if lora is None:
+            return y
+        A, B = l["lora"][proj]
+        x2, y2 = x.reshape(-1, x.shape[-1]), y.view(-1, y.shape[-1])
+        ops.fast.lora_expand_(y2, ops.fast.lora_shrink(x2, A, *lora), B, self.lora_scale, *lora)
+        return y
 
     def _decode_attention_mha(self, qkv, kc, vc, kv_len, position_ids, scale):
         q, k, v = self._split_qkv(qkv, position_ids)
@@ -495,19 +666,22 @@ class DecoderLM:
             return ops.fast.linear_decode(x, self.head_w, None)
         return ops.fast.linear(x, self.head_w, self.head_b)
 
-    def _layers(self, x, position_ids, cache, attend):
+    def _layers(self, x, position_ids, cache, attend, lora=None):
         """The transformer blocks over x [B, T, H].  `attend(q, k, v, kc, vc)` writes a layer's new K/V to its cache
-        and returns the attention output of q [B, T, kv_local, G, D]."""
+        and returns the attention output of q [B, T, kv_local, G, D].  `lora` (see `forward_1d`) adds the adapters'
+        deltas after every targeted projection, before the all-reduce of a row-parallel one."""
         B, T = x.shape[:2]
         for l, (kc, vc) in zip(self.layers, cache):
             h = ops.fast.norm_rows(x, l["ln1"])
-            q, k, v = self._split_qkv(l["qkv"](h).view(B, T, self.kv_local, self.G + 2, self.D), position_ids)
-            a = l["out"](attend(q, k, v, kc, vc).reshape(B, T, self.nh_local * self.D))
+            qkv = self._lora(lora, l, "qkv", h, l["qkv"](h))
+            q, k, v = self._split_qkv(qkv.view(B, T, self.kv_local, self.G + 2, self.D), position_ids)
+            o = attend(q, k, v, kc, vc).reshape(B, T, self.nh_local * self.D)
+            a = self._lora(lora, l, "out", o, l["out"](o))
             if self.cfg.parallel_block:             # x + attn(ln(x)) + mlp(ln(x)): one all-reduce for both branches
                 x = x + self._all_reduce(a + self._mlp(l, h))
                 continue
             x = x + self._all_reduce(a)
-            x = x + self._all_reduce(self._mlp(l, ops.fast.norm_rows(x, l["ln2"])))
+            x = x + self._all_reduce(self._mlp(l, ops.fast.norm_rows(x, l["ln2"]), lora=lora))
         return x
 
     def forward(self, input_ids: torch.Tensor, position_ids: torch.Tensor, cache, cache_len: int,
@@ -568,7 +742,8 @@ class DecoderLM:
                    ctx_len: torch.Tensor, cache, max_ctx: int, logit_index: torch.Tensor,
                    block_table: Optional[torch.Tensor] = None, block_size: Optional[int] = None,
                    chunks: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None,
-                   n_prefill: int = 0) -> torch.Tensor:
+                   n_prefill: int = 0,
+                   lora: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None) -> torch.Tensor:
         """One iteration over a flat batch of T tokens that belong to different sequences (new prompts and running
         decodes mixed).  input_ids/position/slot: int64 [T]; seq_start/ctx_len: int32 [T] (see KVCacheManager.
         prepare_inputs).  K/V of every token go to cache row `slot`; attention reads each sequence's rows in place.
@@ -579,6 +754,8 @@ class DecoderLM:
         PagedKVCacheManager.prepare_inputs) and `n_prefill` their total token count: those tokens, which come first,
         attend through `ops.paged_prefill_attention`, the decode and padding tokens after them through
         `ops.ragged_attention`.
+        `lora` = (rows, seg_start, seg_slot) int32 (`ops.lora_shrink`): the batch rows that carry an adapter grouped
+        by adapter slot; those rows get the adapter's delta after every targeted projection.  None = the base model.
         Returns logits [len(logit_index), V_local] of the rows in `logit_index` (the last token of every sequence).
         (reference: OPTForLMModule.__call__ of opt_model_1d.py:378 with fused_mmha)"""
         T = input_ids.shape[0]
@@ -603,7 +780,8 @@ class DecoderLM:
             return torch.cat([o, r])
 
         # one batch row of T tokens
-        x = self._layers(self._embed(input_ids.view(1, T), position.view(1, T)), position.view(1, T), cache, attend)
+        x = self._layers(self._embed(input_ids.view(1, T), position.view(1, T)), position.view(1, T), cache, attend,
+                         lora)
         if logit_index.numel() == 0:
             return x.new_empty(0, self.V_local)
         return self._head(x[0].index_select(0, logit_index))

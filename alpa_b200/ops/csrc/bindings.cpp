@@ -395,6 +395,79 @@ Tensor ragged_attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_
   return o;
 }
 
+// Multi-LoRA segments (see lora_sm90.cu): rows / seg_start / seg_slot are contiguous int32 CUDA [Tl] / [S + 1] / [S].
+static ab::LoraArgs lora_args(const Tensor& w, const Tensor& rows, const Tensor& seg_start, const Tensor& seg_slot,
+                              const char* op) {
+  for (const Tensor* t : {&rows, &seg_start, &seg_slot})
+    TORCH_CHECK(t->scalar_type() == at::kInt && t->is_contiguous() && t->dim() == 1 && t->device() == w.device(), op,
+                ": rows / seg_start / seg_slot must be contiguous int32 tensors on the adapters' device");
+  TORCH_CHECK(seg_start.numel() == seg_slot.numel() + 1, op, ": seg_start needs one entry more than seg_slot");
+  TORCH_CHECK(w.dim() == 3 && w.is_contiguous() && w.scalar_type() == at::kBFloat16 && aligned(w.data_ptr(), 16), op,
+              ": adapters must be contiguous, 16-byte aligned bf16 [slots, ., .]");
+  TORCH_CHECK(rows.numel() <= INT32_MAX && w.numel() > 0, op, ": too many rows or no adapter slot");
+  ab::LoraArgs a;
+  a.w = bf16_ptr(w);
+  a.rows = rows.data_ptr<int>();
+  a.seg_start = seg_start.data_ptr<int>();
+  a.seg_slot = seg_slot.data_ptr<int>();
+  a.Tl = (int)rows.numel();
+  a.S = (int)seg_slot.numel();
+  return a;
+}
+
+static void check_lora_rows(const Tensor& t, int64_t cols, const char* op, const char* name) {
+  TORCH_CHECK(t.dim() == 2 && t.scalar_type() == at::kBFloat16 && t.stride(1) == 1 && t.size(1) == cols &&
+                  t.stride(0) % 8 == 0 && aligned(t.data_ptr(), 16),
+              op, ": ", name, " must be bf16 [rows, ", cols, "] with unit inner stride, 16-byte aligned rows");
+}
+
+// y [splits, Tl, R] fp32: split p's partial of x[rows[i]] . A[slot]^T; lora_expand_ sums the splits.
+Tensor lora_shrink(const Tensor& x, const Tensor& A, const Tensor& rows, const Tensor& seg_start,
+                   const Tensor& seg_slot) {
+  ab::LoraArgs a = lora_args(A, rows, seg_start, seg_slot, "lora_shrink");
+  a.R = (int)A.size(1);
+  a.K = (int)A.size(2);
+  TORCH_CHECK(a.R % 8 == 0 && a.R <= ab::kLoraMaxRank && a.K % 8 == 0, "lora_shrink: R must be a multiple of 8 up to ",
+              ab::kLoraMaxRank, " and K a multiple of 8");
+  check_lora_rows(x, a.K, "lora_shrink", "x");
+  TORCH_CHECK(x.device() == A.device(), "lora_shrink: x and A on different devices");
+  c10::cuda::CUDAGuard guard(x.device());
+  a.x = bf16_ptr(x);
+  a.ldx = x.stride(0);
+  a.splits = ab_lora_splits(&a);
+  Tensor y = torch::empty({a.splits, a.Tl, a.R}, x.options().dtype(at::kFloat));
+  a.y = y.data_ptr<float>();
+  AB_CHECK_RC(ab_lora_shrink(&a, cur_stream()), "ab_lora_shrink");
+  g_launches += 1;
+  return y;
+}
+
+// out[rows[i]] += scale[slot] * (sum_p y[p, i]) . B[slot]^T, in place, rounded once to bf16.
+void lora_expand_(const Tensor& out, const Tensor& y, const Tensor& B, const Tensor& scale, const Tensor& rows,
+                  const Tensor& seg_start, const Tensor& seg_slot) {
+  ab::LoraArgs a = lora_args(B, rows, seg_start, seg_slot, "lora_expand_");
+  a.N = (int)B.size(1);
+  a.R = (int)B.size(2);
+  TORCH_CHECK(a.R % 8 == 0 && a.R <= ab::kLoraMaxRank && a.N % 8 == 0, "lora_expand_: R must be a multiple of 8 up to ",
+              ab::kLoraMaxRank, " and N a multiple of 8");
+  check_lora_rows(out, a.N, "lora_expand_", "out");
+  TORCH_CHECK(y.dim() == 3 && y.scalar_type() == at::kFloat && y.is_contiguous() && y.size(1) == a.Tl &&
+                  y.size(2) == a.R && y.size(0) >= 1 && y.device() == B.device(),
+              "lora_expand_: y must be contiguous fp32 [splits, Tl, R]");
+  TORCH_CHECK(scale.scalar_type() == at::kFloat && scale.is_contiguous() && scale.numel() == B.size(0) &&
+                  scale.device() == B.device(),
+              "lora_expand_: scale must be contiguous fp32 [slots]");
+  TORCH_CHECK(out.device() == B.device(), "lora_expand_: out and B on different devices");
+  c10::cuda::CUDAGuard guard(out.device());
+  a.out = reinterpret_cast<__nv_bfloat16*>(out.data_ptr());
+  a.ldo = out.stride(0);
+  a.y = const_cast<float*>(y.data_ptr<float>());
+  a.scale = scale.data_ptr<float>();
+  a.splits = (int)y.size(0);
+  AB_CHECK_RC(ab_lora_expand(&a, cur_stream()), "ab_lora_expand");
+  g_launches += 1;
+}
+
 // Causal prefill of query chunks against a paged bf16 cache (see paged_prefill_sm90.cu).  q: [T, heads, D] or the
 // grouped view [T, kv_heads, group, D]; chunk c's keys are read through row c of the block table.  `max_keys` bounds
 // chunk_pos + chunk_len of every chunk (the descriptors stay on the device); the table must cover it.
@@ -1371,6 +1444,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("paged_prefill_attention", &paged_prefill_attention, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"),
         py::arg("block_table"), py::arg("block_size"), py::arg("chunk_start"), py::arg("chunk_len"),
         py::arg("chunk_pos"), py::arg("scale"), py::arg("max_keys"));
+  m.def("lora_shrink", &lora_shrink, py::arg("x"), py::arg("A"), py::arg("rows"), py::arg("seg_start"),
+        py::arg("seg_slot"));
+  m.def("lora_expand_", &lora_expand_, py::arg("out"), py::arg("y"), py::arg("B"), py::arg("scale"), py::arg("rows"),
+        py::arg("seg_start"), py::arg("seg_slot"));
   m.def("dropout", &dropout);
   m.def("embedding_fwd", &embedding_fwd);
   m.def("embedding_bwd_", &embedding_bwd_);

@@ -184,6 +184,23 @@ struct DecodeAttnArgs {
   long long scale_stride_b = 0, scale_stride_h = 0;
 };
 
+// Multi-LoRA shrink / expand over segments of a ragged token batch (lora_sm90.cu).  Segment s is batch rows
+// rows[seg_start[s] .. seg_start[s + 1]) and uses adapter slot seg_slot[s]; rows, seg_start and seg_slot are trusted
+// like the block table (the batch assembly builds them).  A row of x / out that no segment lists is never touched.
+constexpr int kLoraMaxRank = 192;  // R: up to three stacked projections of rank 64
+struct LoraArgs {
+  const __nv_bfloat16* x = nullptr;      // shrink input [*, K], row stride ldx
+  const __nv_bfloat16* w = nullptr;      // shrink: A [slots, R, K]; expand: B [slots, N, R]
+  float* y = nullptr;                    // [splits, Tl, R] fp32: shrink writes split p's partial, expand sums them
+  __nv_bfloat16* out = nullptr;          // expand: [*, N], row stride ldo, updated in place
+  const float* scale = nullptr;          // expand: [slots]
+  const int* rows = nullptr;             // [Tl]
+  const int* seg_start = nullptr;        // [S + 1]
+  const int* seg_slot = nullptr;         // [S]
+  long long ldx = 0, ldo = 0;
+  int Tl = 0, S = 0, K = 0, N = 0, R = 0, splits = 1;
+};
+
 // Quantising store of bf16 K / V rows into an fp8 cache (kv_cache_sm90.cu).  Source token (b, t) of head h is at
 // k + b * k_stride[0] + t * k_stride[1] + h * k_stride[2] (v with v_stride; D contiguous); it goes to cache row
 // rows[b * T + t], or b * S + start + t when rows is null.  Cache row r of head h: data at (r * H + h) * D, scale at
@@ -251,6 +268,9 @@ int ab_attention_bwd_splits(const ab::AttnArgs* a);  // parts the dK / dV kernel
 int ab_gemv_decode(const ab::GemvArgs* a, cudaStream_t st);
 int ab_ragged_attention(const ab::RaggedAttnArgs* a, cudaStream_t st);
 int ab_paged_prefill(const ab::PagedPrefillArgs* a, cudaStream_t st);
+int ab_lora_splits(const ab::LoraArgs* a);  // K splits of the shrink for these shapes (the partials' first dim)
+int ab_lora_shrink(const ab::LoraArgs* a, cudaStream_t st);
+int ab_lora_expand(const ab::LoraArgs* a, cudaStream_t st);
 int ab_decode_attention(const ab::DecodeAttnArgs* a, cudaStream_t st);
 int ab_decode_attention_rows(const ab::DecodeAttnArgs* a);  // CTA rows per sequence (kv_heads * group chunks)
 int ab_decode_attention_chunk(const ab::DecodeAttnArgs* a);  // query heads per CTA (partials per row and split)

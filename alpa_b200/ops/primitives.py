@@ -23,7 +23,7 @@ __all__ = [
     "attention_gqa_packed_bwd", "embedding", "embedding_bwd",
     "cross_entropy", "cross_entropy_bwd", "fused_adamw_", "pipeline_marker",
     "bmm", "moe_dispatch", "moe_combine", "moe_combine_wgrad", "moe_top2_route", "linear_fp8", "linear_decode", "RMSNormArgs", "decode_attention", "decode_attention_gqa", "ragged_attention",
-    "paged_prefill_attention",
+    "paged_prefill_attention", "lora_shrink", "lora_expand_",
     "Fp8KV", "kv_cache_store", "kv_cache_load", "kv_cache_nbytes",
     "attention_cached", "attention_cached_", "quantize_mxfp8", "dequantize_mxfp8", "linear_mxfp8", "mx_pack_scale_atoms",
     "mx_unpack_scale_atoms", "pack_tiles", "unpack_tiles", "packed_nbytes",
@@ -1240,6 +1240,64 @@ def paged_prefill_attention(q: Tensor, k_cache: Tensor, v_cache: Tensor, block_t
         p = torch.softmax(s, dim=-1)
         o[s0:s0 + n] = torch.einsum("hij,jhd->ihd", p, v).to(q.dtype)
     return o
+
+
+# =================================================================================================
+# multi-LoRA segments (serving many adapters over one base model)
+# =================================================================================================
+LORA_MAX_RANK = 192         # R of the kernels: up to three stacked projections of rank 64
+
+
+def _lora_unsupported(rows_mat: Tensor, w: Tensor, R: int, inner: int) -> Optional[str]:
+    """Why the LoRA kernels cannot take these operands, or None.  rows_mat: x (shrink) or out (expand), w: A or B
+    with rank R and other dimension `inner` (K of A, N of B)."""
+    if R % 8 or R > LORA_MAX_RANK or inner % 8:
+        return "LoRA rank not a multiple of 8 up to 192, or K / N not a multiple of 8"
+    if rows_mat.dim() != 2 or rows_mat.stride(-1) != 1 or rows_mat.stride(0) % 8 or rows_mat.data_ptr() % 16:
+        return "LoRA rows not 16-byte aligned"
+    if not w.is_contiguous() or w.data_ptr() % 16:
+        return "LoRA adapters not contiguous"
+    return None
+
+
+def _lora_segments(rows: Tensor, seg_start: Tensor, seg_slot: Tensor):
+    starts = seg_start.tolist()
+    for s, slot in enumerate(seg_slot.tolist()):
+        yield slot, starts[s], starts[s + 1], rows[starts[s]:starts[s + 1]].long()
+
+
+@torch.library.custom_op("alpa_b200::lora_shrink", mutates_args=())
+def lora_shrink(x: Tensor, A: Tensor, rows: Tensor, seg_start: Tensor, seg_slot: Tensor) -> Tensor:
+    """LoRA shrink over segments of a token batch.  x: [T, K]; A: [slots, R, K]; rows int32 [Tl] (batch rows grouped
+    by segment), seg_start int32 [S + 1], seg_slot int32 [S]: segment s is rows[seg_start[s]:seg_start[s + 1]] and uses
+    adapter A[seg_slot[s]].  Returns fp32 partials y [P, Tl, R] whose sum over P is x[rows[i]] . A[slot]^T (the kernel
+    splits K into P parts, the reference returns P = 1); `lora_expand_` takes them as they are.  Rows of y outside
+    every segment are undefined."""
+    if C := _kernels("lora_shrink", x, A, unsupported=lambda: _lora_unsupported(x, A, A.shape[1], A.shape[2])):
+        return C.lora_shrink(x, A, rows, seg_start, seg_slot)
+    y = torch.zeros(1, rows.shape[0], A.shape[1], dtype=torch.float32, device=x.device)
+    for slot, b, e, r in _lora_segments(rows, seg_start, seg_slot):
+        y[0, b:e] = x[r].float() @ A[slot].float().T
+    return y
+
+
+@lora_shrink.register_fake
+def _(x, A, rows, seg_start, seg_slot):
+    return x.new_empty(1, rows.shape[0], A.shape[1], dtype=torch.float32)
+
+
+@torch.library.custom_op("alpa_b200::lora_expand_", mutates_args=("out",))
+def lora_expand_(out: Tensor, y: Tensor, B: Tensor, scale: Tensor, rows: Tensor, seg_start: Tensor,
+                 seg_slot: Tensor) -> None:
+    """LoRA expand, in place: out[rows[i]] = out[rows[i]] + scale[slot] * (y[:, i].sum(0) . B[slot]^T), rounded once
+    to out's dtype.  out: [T, N]; y: [P, Tl, R] fp32 (`lora_shrink`); B: [slots, N, R]; scale: fp32 [slots]
+    (lora_alpha / r).  A row of out that no segment lists is neither read nor written."""
+    if C := _kernels("lora_expand_", out, B, unsupported=lambda: _lora_unsupported(out, B, B.shape[2], B.shape[1])):
+        C.lora_expand_(out, y, B, scale, rows, seg_start, seg_slot)
+        return
+    ys = y.sum(0)
+    for slot, b, e, r in _lora_segments(rows, seg_start, seg_slot):
+        out[r] = (out[r].float() + scale[slot].float() * (ys[b:e] @ B[slot].float().T)).to(out.dtype)
 
 
 # =================================================================================================

@@ -13,6 +13,11 @@ and when the blocks run out the most recently admitted sequences are preempted a
 `prefix_caching=True` as well, full blocks are shared between sequences whose token prefixes are equal: a new or
 re-admitted prompt starts from the longest cached chain of blocks matching it and prefills only the rest, and that
 suffix attends to the cached keys through `ops.paged_prefill_attention` (sm_90a kernel).
+
+A prompt may name a LoRA adapter loaded into the model (`DecoderLM.load_lora`; `enter_prompts(loras=...)` takes its load
+id).  `next()` then also lists the batch rows that carry an adapter, grouped by adapter slot, and the model adds each
+adapter's delta to its rows (`ops.lora_shrink` / `ops.lora_expand_`).  With prefix caching, an adapter's blocks are
+shared only between its own sequences (the load id is the block manager's namespace).
 """
 from __future__ import annotations
 
@@ -36,8 +41,9 @@ class PromptStatus(Enum):
 class Prompt:
     """One sequence travelling through the pool."""
 
-    def __init__(self, input_ids: Sequence[int], sentence_id: int, max_length: int = 2048):
+    def __init__(self, input_ids: Sequence[int], sentence_id: int, max_length: int = 2048, lora: Optional[int] = None):
         self.input_ids = list(input_ids)
+        self.lora = lora                             # LoRA load id, None = the base model; kept across preemptions
         self.sentence_id = sentence_id
         self.max_length = max_length                 # prompt + generated, also the cache reservation
         self.status = PromptStatus.PROMPT
@@ -106,9 +112,15 @@ class IterationLevelInputPool:
     the sampled token of every sequence in that iteration."""
 
     def __init__(self, config: InputPoolConfig, pad_token_id: int = 1, eos_token_id: int = 2,
-                 max_length: Optional[int] = None, max_new_tokens: Optional[int] = None):
+                 max_length: Optional[int] = None, max_new_tokens: Optional[int] = None,
+                 model: Optional[DecoderLM] = None):
+        """`model`: the model the pool's batches run on; prompts with a LoRA adapter need it (it maps load ids to
+        slots and refuses to unload an adapter a queued or running prompt of this pool uses)."""
         from alpa_b200 import _planner
         self.config = config
+        self.model = model
+        if model is not None:
+            model._lora_pools.add(self)
         self.batch_size = config.batch_size
         self.cache_size = config.cache_size
         self.max_length = max_length
@@ -178,10 +190,18 @@ class IterationLevelInputPool:
         return sum(pending) <= self.batch_size - len(self.wip) and blocks <= self.cache_manager.num_free_blocks
 
     def enter_prompts(self, input_sequences: Sequence[Sequence[int]],
-                      max_lengths: Optional[Sequence[int]] = None) -> List[int]:
-        """Queue prompts; `max_lengths[i]` (prompt + generated) overrides the pool-wide limits for sequence i."""
+                      max_lengths: Optional[Sequence[int]] = None,
+                      loras: Optional[Sequence[Optional[int]]] = None) -> List[int]:
+        """Queue prompts; `max_lengths[i]` (prompt + generated) overrides the pool-wide limits for sequence i, and
+        `loras[i]` is the load id (`DecoderLM.lora_id`) of its LoRA adapter, None for the base model."""
         ids = []
         paged = self.block_size is not None
+        loras = [None] * len(input_sequences) if loras is None else list(loras)
+        if len(loras) != len(input_sequences):
+            raise ValueError("loras needs one entry per prompt")
+        for lid in loras:
+            if lid is not None and (self.model is None or lid not in self.model.lora_slot_of):
+                raise ValueError(f"no LoRA adapter with load id {lid} is loaded in this pool's model")
         for i, seq in enumerate(input_sequences):
             if len(seq) == 0:
                 raise ValueError("empty prompt")
@@ -204,7 +224,7 @@ class IterationLevelInputPool:
                 raise ValueError(f"prompt needs {need} cache slots, the cache has {self.cache_size}")
             sid = self._next_id
             self._next_id += 1
-            self.todo.append(Prompt(seq, sid, max_length=need))
+            self.todo.append(Prompt(seq, sid, max_length=need, lora=loras[i]))
             ids.append(sid)
         return ids
 
@@ -235,7 +255,9 @@ class IterationLevelInputPool:
                                                 [p.sentence_id for p in decoding], width, self.pad_slot)
         tokens = tokens + [self.pad] * (width - len(tokens))
         self._current = admitted + decoding
-        return {"input_ids": tokens, "num_new_prompts": len(admitted), "num_decoding": len(decoding), **idx}
+        lora = self._lora_segments([p.lora for p in admitted for _ in range(p.prompt_length)] +
+                                   [p.lora for p in decoding])
+        return {"input_ids": tokens, "num_new_prompts": len(admitted), "num_decoding": len(decoding), **idx, **lora}
 
     def _width(self, n_tokens: int) -> int:
         mult = max(1, self.config.pad_multiple or 8)
@@ -277,7 +299,7 @@ class IterationLevelInputPool:
                 # admission (or re-admission after a preemption): start from the cached blocks of its prefix; cached
                 # blocks it takes a reference on were counted as free
                 before = cm.num_free_blocks
-                hit = cm.match_prefix(p.sentence_id, p.fill_ids)
+                hit = cm.match_prefix(p.sentence_id, p.fill_ids, p.lora or 0)
                 free -= before - cm.num_free_blocks
                 if free < 0:                           # the decoding sequences need those blocks: retry later
                     cm.free(p.sentence_id)
@@ -300,7 +322,7 @@ class IterationLevelInputPool:
         ends = []
         for p, take in chunks:
             if not cm.has(p.sentence_id):
-                cm.allocate(p.sentence_id)
+                cm.allocate(p.sentence_id, p.lora or 0)
                 self._admit(p)
             ends.append(p.filled + take == len(p.fill_ids))
         tokens = [t for p, take in chunks for t in p.fill_ids[p.filled:p.filled + take]]
@@ -320,7 +342,29 @@ class IterationLevelInputPool:
         self.peak_blocks_used = max(self.peak_blocks_used, cm.num_blocks - cm.num_free_blocks)
         tokens = tokens + [self.pad] * (width - len(tokens))
         self._current = [p for (p, _), end in zip(chunks, ends) if end] + decoding
-        return {"input_ids": tokens, "num_new_prompts": sum(ends), "num_decoding": len(decoding), **idx}
+        lora = self._lora_segments([p.lora for p, take in chunks for _ in range(take)] + [p.lora for p in decoding])
+        return {"input_ids": tokens, "num_new_prompts": sum(ends), "num_decoding": len(decoding), **idx, **lora}
+
+    def _lora_segments(self, row_loras: List[Optional[int]]) -> Dict:
+        """`lora_rows` / `lora_seg_start` / `lora_seg_slot` (`ops.lora_shrink`) of the batch rows that carry an
+        adapter, one segment per adapter in slot order; empty when no row does."""
+        if all(lid is None for lid in row_loras):
+            return {}
+        by_slot: Dict[int, List[int]] = {}
+        for row, lid in enumerate(row_loras):
+            if lid is not None:
+                by_slot.setdefault(self.model.lora_slot_of[lid], []).append(row)
+        rows, starts, slots = [], [0], []
+        for slot in sorted(by_slot):
+            rows += by_slot[slot]
+            starts.append(len(rows))
+            slots.append(slot)
+        return {"lora_rows": rows, "lora_seg_start": starts, "lora_seg_slot": slots}
+
+    def uses_lora(self, load_id: int) -> bool:
+        """Does a queued, running or just-batched prompt use this adapter?"""
+        live = list(self.todo) + list(self.wip.values()) + list(self._current or [])
+        return any(p.lora == load_id for p in live)
 
     def _admit(self, p: Prompt):
         self._admissions += 1
@@ -427,6 +471,9 @@ class SequenceGenerator:
         ids, pos, slot, seq_start, ctx_len, logit_index, block_table = self._to_dev(batch)
         m = self.model
         paged = {} if block_table is None else {"block_table": block_table, "block_size": pool.block_size}
+        if "lora_rows" in batch:
+            paged["lora"] = tuple(torch.tensor(batch[k], dtype=torch.int32, device=m.device)
+                                  for k in ("lora_rows", "lora_seg_start", "lora_seg_slot"))
         if "chunk_len" in batch and batch["chunk_len"]:
             dev = m.device
             paged["chunks"] = tuple(torch.tensor(batch[k], dtype=torch.int32, device=dev)
@@ -446,12 +493,15 @@ class SequenceGenerator:
         return n
 
     def generate(self, input_ids: Sequence[Sequence[int]], max_length: Optional[int] = None,
-                 max_new_tokens: Optional[int] = None, **unused) -> List[List[int]]:
-        """All prompts enter at once and drain through the iteration loop (reference: generate_by_batch)."""
+                 max_new_tokens: Optional[int] = None, loras: Optional[Sequence[Optional[str]]] = None,
+                 **unused) -> List[List[int]]:
+        """All prompts enter at once and drain through the iteration loop (reference: generate_by_batch).  `loras[i]`
+        names the LoRA adapter of prompt i (`DecoderLM.load_lora`), None for the base model."""
         cfg = self.model.cfg
+        ids = None if loras is None else [None if n is None else self.model.lora_id(n) for n in loras]
         pool = IterationLevelInputPool(self.pool_config, pad_token_id=cfg.pad_token_id, eos_token_id=2,
-                                       max_length=max_length, max_new_tokens=max_new_tokens)
-        pool.enter_prompts(input_ids)
+                                       max_length=max_length, max_new_tokens=max_new_tokens, model=self.model)
+        pool.enter_prompts(input_ids, loras=ids)
         while not pool.is_finished():
             self.step(pool)
         self.last_latency = pool.get_latency()

@@ -421,6 +421,35 @@ def load_params_np(cfg: OPTConfig, path: str) -> Dict[str, torch.Tensor]:
     return p
 
 
+def load_lora_np(cfg: OPTConfig, path: str):
+    """A PEFT LoRA adapter directory in the one-file-per-tensor form `load_params_np` reads: `adapter_config.json` (r,
+    lora_alpha, target_modules) and one .npy file per tensor, named by PEFT (`base_model.model.model.layers.N.
+    self_attn.q_proj.lora_A.weight`, with or without a .npy suffix).  Returns (tensors, alpha, r) for
+    `DecoderLM.load_lora(name, *load_lora_np(cfg, path))`; raises ValueError for a target the model cannot serve."""
+    import json
+    import os
+
+    import numpy as np
+
+    from alpa_b200.model.opt_model import LORA_TARGETS
+    with open(os.path.join(path, "adapter_config.json")) as f:
+        conf = json.load(f)
+    r, alpha = int(conf["r"]), float(conf.get("lora_alpha", conf["r"]))
+    targets = LORA_TARGETS.get(cfg.arch)
+    if targets is None:
+        raise ValueError(f"LoRA adapters are served for Llama and OPT models, not {cfg.arch!r}")
+    mods = conf.get("target_modules") or []
+    mods = [mods] if isinstance(mods, str) else mods
+    bad = sorted(set(mods) - set(targets))
+    if bad:
+        raise ValueError(f"unsupported LoRA target_modules {bad} for {cfg.arch!r} (supported: {sorted(targets)})")
+    tensors = {}
+    for name in os.listdir(path):
+        if ".lora_A" in name or ".lora_B" in name:
+            tensors[name.removesuffix(".npy")] = torch.from_numpy(np.load(os.path.join(path, name)))
+    return tensors, alpha, r
+
+
 def _load_bloom_params(cfg: OPTConfig, ld) -> Dict[str, torch.Tensor]:
     """Hugging Face BLOOM names (reference: load_params_np of bloom_model.py).  `query_key_value` rows are ordered
     [head, (q, k, v), D]."""

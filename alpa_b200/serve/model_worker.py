@@ -42,6 +42,7 @@ class GenerateItem:
     top_p: float = 1.0
     min_tokens: int = 0
     echo: bool = True
+    lora: Optional[int] = None             # LoRA load id (DecoderLM.lora_id), None = the base model
 
 
 @dataclass
@@ -51,6 +52,7 @@ class LogprobsItem:
     top_k: int
     future: asyncio.Future
     enqueue_time: float = field(default_factory=time.time)
+    lora: Optional[int] = None
 
 
 class LangModelWorker:
@@ -74,7 +76,7 @@ class LangModelWorker:
         self.model = model
         self.engine = SequenceGenerator(model, pool_config)
         self.pool = IterationLevelInputPool(self.engine.pool_config, pad_token_id=model.cfg.pad_token_id,
-                                            eos_token_id=eos_token_id)
+                                            eos_token_id=eos_token_id, model=model)
         self.max_new_tokens_limit = max_new_tokens_limit
         group_weights = dict(group_weights or {DEFAULT_GROUP: 1.0, API_KEY_GROUP: 4.0})
         inner = {g: deque() for g in group_weights}
@@ -98,9 +100,12 @@ class LangModelWorker:
         self._wake.set()
 
     async def completions(self, prompt_ids: Sequence[int], max_tokens: int = 16, api_key: Optional[str] = None,
-                          temperature: float = 0.0, top_p: float = 1.0, min_tokens: int = 0, echo: bool = True) -> Dict:
+                          temperature: float = 0.0, top_p: float = 1.0, min_tokens: int = 0, echo: bool = True,
+                          lora: Optional[str] = None) -> Dict:
         """`temperature` 0 = greedy, > 0 = sample from softmax(logits / temperature) restricted to the smallest token
-        set of mass `top_p`; no end-of-sequence before `min_tokens` new tokens; `echo` keeps the prompt in "ids"."""
+        set of mass `top_p`; no end-of-sequence before `min_tokens` new tokens; `echo` keeps the prompt in "ids";
+        `lora` names a loaded LoRA adapter (ValueError for an unknown one), None = the base model."""
+        lid = None if lora is None else self.model.lora_id(lora)
         if not (0.0 <= float(top_p) <= 1.0) or float(temperature) < 0.0:
             raise ValueError("need 0 <= top_p <= 1 and temperature >= 0")
         if len(prompt_ids) == 0:
@@ -112,13 +117,15 @@ class LangModelWorker:
         fut = asyncio.get_running_loop().create_future()
         self._enqueue(GenerateItem(self._uid, list(map(int, prompt_ids)), max_tokens, fut,
                                    temperature=float(temperature), top_p=float(top_p),
-                                   min_tokens=min(int(min_tokens), max_tokens - 1), echo=bool(echo)), api_key)
+                                   min_tokens=min(int(min_tokens), max_tokens - 1), echo=bool(echo), lora=lid), api_key)
         return await fut
 
-    async def logprobs(self, prompt_ids: Sequence[int], top_k: int = 1, api_key: Optional[str] = None) -> Dict:
+    async def logprobs(self, prompt_ids: Sequence[int], top_k: int = 1, api_key: Optional[str] = None,
+                       lora: Optional[str] = None) -> Dict:
+        lid = None if lora is None else self.model.lora_id(lora)
         self._uid += 1
         fut = asyncio.get_running_loop().create_future()
-        self._enqueue(LogprobsItem(self._uid, list(map(int, prompt_ids)), top_k, fut), api_key)
+        self._enqueue(LogprobsItem(self._uid, list(map(int, prompt_ids)), top_k, fut, lora=lid), api_key)
         return await fut
 
     # ---- request plumbing (reference: launch_model_worker.py normalize_prompts:231, check_max_length_limit:394,
@@ -182,7 +189,7 @@ class LangModelWorker:
 
     async def handle_request(self, request) -> Dict:
         """{"prompt" | "prompt_ids": str | [str] | [int] | [[int]], "max_tokens": n, "api_key": ..., "logprobs": bool,
-        "top_k": k}.  One prompt -> the result dict; several prompts -> {"choices": [result, ...]} (served
+        "top_k": k, "lora": adapter name}.  One prompt -> the result dict; several prompts -> {"choices": [result, ...]} (served
         concurrently by the continuous-batching loop)."""
         obj = request.json() if hasattr(request, "json") else dict(request)
         api_key = self.get_authorization(obj, request)
@@ -197,8 +204,11 @@ class LangModelWorker:
         want_logprobs = bool(obj.get("logprobs")) or path.endswith("/logprobs")
         if "stop" in obj:
             raise NotImplementedError("The stop argument is not implemented")
+        lora = obj.get("lora")
+        if lora is not None:
+            self.model.lora_id(str(lora))                    # an unknown adapter fails the request before queueing
         if want_logprobs:
-            coros = [self.logprobs(p, int(obj.get("top_k", 1)), api_key) for p in prompts]
+            coros = [self.logprobs(p, int(obj.get("top_k", 1)), api_key, lora) for p in prompts]
         else:
             # greedy unless the request asks for sampling (reference: temperature / top_p rounded to one decimal,
             # launch_model_worker.py:276-277)
@@ -207,7 +217,7 @@ class LangModelWorker:
                 temperature = 1.0
             top_p = round(float(obj.get("top_p", 1.0)), 1)
             coros = [self.completions(p, max_tokens, api_key, temperature, top_p, int(obj.get("min_tokens", 0)),
-                                      bool(obj.get("echo", True))) for p in prompts]
+                                      bool(obj.get("echo", True)), lora) for p in prompts]
         results = await asyncio.gather(*coros)
         if self.tokenizer is not None:
             for r in results:
@@ -255,7 +265,8 @@ class LangModelWorker:
                 self.request_queue.put_nowait_special(lambda s, x: s.appendleft(x), entry)
                 self.request_queue.task_done()            # the re-queued entry is counted again by put_nowait_special
                 return None
-            sid = pool.enter_prompts([item.prompt_ids], max_lengths=[need])[0]     # stops after item.max_tokens tokens
+            # stops after item.max_tokens tokens
+            sid = pool.enter_prompts([item.prompt_ids], max_lengths=[need], loras=[item.lora])[0]
             self._running[sid] = item
         return None
 
@@ -264,7 +275,15 @@ class LangModelWorker:
         ids = torch.tensor([item.prompt_ids], dtype=torch.long, device=m.device)
         T = ids.shape[1]
         pos = torch.arange(T, device=m.device)[None]
-        logits = m.gather_logits(m.forward(ids, pos, m.init_cache(1, T), 0, last_only=False)).float()
+        if item.lora is None:
+            logits = m.gather_logits(m.forward(ids, pos, m.init_cache(1, T), 0, last_only=False)).float()
+        else:
+            # adapters are served on the ragged path: the prompt as one sequence in a slot cache of its own
+            i32 = lambda t: t.to(torch.int32)  # noqa: E731
+            lora = (i32(pos[0]), torch.tensor([0, T], dtype=torch.int32, device=m.device),
+                    torch.tensor([m.lora_slot_of[item.lora]], dtype=torch.int32, device=m.device))
+            logits = m.gather_logits(m.forward_1d(ids[0], pos[0], pos[0], i32(pos[0] * 0), i32(pos[0] + 1),
+                                                  m.init_cache_1d(T), T, pos[0], lora=lora))[None].float()
         lp_all = torch.log_softmax(logits[0], dim=-1)
         lp = lp_all[:-1]
         tok = lp.gather(-1, ids[0, 1:, None])[:, 0]
@@ -348,4 +367,4 @@ class LangModelWorker:
                         item.future.set_exception(e)
                 self._running.clear()
                 self.pool = pool = IterationLevelInputPool(self.engine.pool_config, pad_token_id=self.model.cfg.pad_token_id,
-                                                           eos_token_id=pool.eos)
+                                                           eos_token_id=pool.eos, model=self.model)

@@ -25,6 +25,13 @@ Prefix caching off against on, every request starting with the same 1024-token p
 `--prefix-caching` runs every paged block size with caching off and on, alternated in one process; each run reports
 its time to first token (p50 / p99, from the moment all requests are queued), the prompt tokens found in the cache
 and the prompt tokens computed.
+
+Multi-LoRA serving, the base model against 8 and 32 rank-16 adapters spread round robin over the requests:
+
+    python scripts/bench_serving_continuous.py --model llama-3-8b --kv-block-size 16 --loras 0,8,32
+
+`--loras` runs every mode once per adapter count, alternated in one process on one model (0 = no adapter).  The
+adapters are random (every target of the architecture), so the outputs are meaningless and only the speed counts.
 """
 import argparse
 import json
@@ -62,6 +69,9 @@ def main():
                    help="run every paged block size with prefix caching off and on")
     p.add_argument("--shared-prefix-tokens", type=int, default=0,
                    help="every prompt starts with the same preamble of this many tokens")
+    p.add_argument("--loras", default="0",
+                   help="comma list of LoRA adapter counts spread over the requests, run alternately; 0 = base model")
+    p.add_argument("--lora-rank", type=int, default=16)
     args = p.parse_args()
     from alpa_b200 import ops
     from alpa_b200.model.opt_model import DecoderLM, get_config
@@ -72,7 +82,11 @@ def main():
     cfg = get_config(args.model, dtype=dtype, weight_dtype=args.weight_dtype, kv_cache_dtype=args.kv_cache_dtype)
     if args.layers:
         cfg.num_hidden_layers = args.layers
+    lora_counts = [int(n) for n in args.loras.split(",")]
+    cfg.max_loras, cfg.max_lora_rank = max(lora_counts), args.lora_rank
     model = DecoderLM(cfg, device=dev, seed=0)
+    for i in range(cfg.max_loras):
+        model.load_lora(f"a{i}", random_lora(cfg, args.lora_rank, seed=i), 2.0 * args.lora_rank, args.lora_rank)
     rnd = random.Random(0)
     preamble = [rnd.randint(4, cfg.vocab_size - 1) for _ in range(args.shared_prefix_tokens)]
     reqs = [(preamble + [rnd.randint(4, cfg.vocab_size - 1)
@@ -90,19 +104,22 @@ def main():
     declared = [len(r[0]) + (args.max_tokens or r[1]) for r in reqs]
     eos = 2
     # a mode is (block size, prefix caching)
-    modes = [(int(b), c) for b in args.kv_block_size.split(",")
-             for c in ((False, True) if args.prefix_caching and int(b) else (False,))]
+    # a mode is (block size, prefix caching, LoRA adapters)
+    modes = [(int(b), c, n) for b in args.kv_block_size.split(",")
+             for c in ((False, True) if args.prefix_caching and int(b) else (False,)) for n in lora_counts]
     engines = {}
-    for bs, caching in modes:
+    for bs, caching, n in modes:
         pc = InputPoolConfig(batch_size=args.batch_tokens, cache_size=cache_tokens, max_cache_per_seq=per_seq,
                              kv_block_size=bs or None, prefix_caching=caching)
-        engines[(bs, caching)] = SequenceGenerator(model, pc)
+        engines[(bs, caching, n)] = SequenceGenerator(model, pc)
 
     def run_continuous(mode):
         eng = engines[mode]
         pool = IterationLevelInputPool(eng.pool_config, pad_token_id=cfg.pad_token_id,
-                                       eos_token_id=eos if args.max_tokens else -1)
-        ids = pool.enter_prompts([r[0] for r in reqs], max_lengths=declared)
+                                       eos_token_id=eos if args.max_tokens else -1, model=model)
+        n = mode[2]
+        loras = [model.lora_id(f"a{i % n}") if n else None for i in range(len(reqs))]
+        ids = pool.enter_prompts([r[0] for r in reqs], max_lengths=declared, loras=loras)
         true_len = {sid: r[1] for sid, r in zip(ids, reqs)}
         stats = {"decode_iterations": 0, "decode_rows": 0, "ttft": {}}
 
@@ -171,9 +188,9 @@ def main():
         "static_padded": {"tokens_per_s": total_new / t_stat, "seconds": t_stat, "batch": args.static_batch,
                           "mean_latency_s": sum(lat_stat) / len(lat_stat), "p90_latency_s": pct(lat_stat, 0.9)},
         "speedup": t_stat / t_cont, "requests": args.requests, "generated_tokens": total_new,
-        "kv_cache": [{"kv_block_size": bs or None, "prefix_caching": caching,
+        "kv_cache": [{"kv_block_size": bs or None, "prefix_caching": caching, "loras": n,
                       "tokens_per_s": total_new / t, "seconds": t, "iterations": it,
-                      "tokens_per_s_runs": [total_new / r[0] for r in results[(bs, caching)]],
+                      "tokens_per_s_runs": [total_new / r[0] for r in results[(bs, caching, n)]],
                       "mean_latency_s": sum(lat) / len(lat), "p90_latency_s": pct(lat, 0.9),
                       "mean_seqs_per_decode_iteration": st["decode_rows"] / max(1, st["decode_iterations"])
                       if args.max_tokens else None,
@@ -182,14 +199,32 @@ def main():
                       "ttft_p99_s": pct(list(st["ttft"].values()), 0.99),
                       "prefix_hit_tokens": pool.prefix_hit_tokens if bs else None,
                       "prefill_tokens_computed": pool.prefill_tokens_computed if bs else None,
-                      "cache_tokens": cache_tokens, "cache_bytes": ops.kv_cache_nbytes(engines[(bs, caching)].cache),
+                      "cache_tokens": cache_tokens, "cache_bytes": ops.kv_cache_nbytes(engines[(bs, caching, n)].cache),
                       "kv_cache_dtype": args.kv_cache_dtype}
-                     for bs, caching in modes
-                     for t, lat, it, pool, st in [min(results[(bs, caching)], key=lambda r: r[0])]],
+                     for bs, caching, n in modes
+                     for t, lat, it, pool, st in [min(results[(bs, caching, n)], key=lambda r: r[0])]],
+        "lora_rank": args.lora_rank if cfg.max_loras else None,
         "shared_prefix_tokens": args.shared_prefix_tokens,
         "declared_max_tokens": args.max_tokens,
         "prompt_len_range": [args.min_prompt, args.max_prompt], "new_tokens_range": [args.min_new, args.max_new],
         "weight_dtype": args.weight_dtype, "device": str(dev), "data": "synthetic prompts, random-init weights"}))
+
+
+def random_lora(cfg, r, seed):
+    """A random adapter on every LoRA target of cfg's architecture, under PEFT's tensor names."""
+    from alpa_b200.model.opt_model import LORA_TARGETS
+    H, I, D = cfg.hidden_size, cfg.ffn_dim, cfg.head_dim
+    dims = {"q_proj": (H, cfg.num_attention_heads * D), "k_proj": (H, cfg.kv_heads * D),
+            "v_proj": (H, cfg.kv_heads * D), "o_proj": (H, H), "out_proj": (H, H), "gate_proj": (H, I),
+            "up_proj": (H, I), "down_proj": (I, H), "fc2": (I, H)}
+    g = torch.Generator().manual_seed(seed)
+    out = {}
+    for i in range(cfg.num_hidden_layers):
+        for mod in LORA_TARGETS[cfg.arch]:
+            k_in, n_out = dims[mod]
+            out[f"layers.{i}.{mod}.lora_A.weight"] = torch.randn(r, k_in, generator=g) / k_in ** 0.5
+            out[f"layers.{i}.{mod}.lora_B.weight"] = torch.randn(n_out, r, generator=g) * 0.01
+    return out
 
 
 if __name__ == "__main__":
